@@ -149,6 +149,31 @@ void spiralOffsets(int w, std::vector<short2>& locs) {
   }
 }
 
+// The kernels that evaluate costs, instantiated for one visibility-mask width (evalCost in derp_cost.cuh).
+struct CostKernels {
+  void (*sweep)(SweepArgs);
+  void (*evalCost)(CostView, const float*, float*, float*, unsigned long long*);
+  void (*proposal)(ProposalArgs);
+  void (*pingPong)(PingPongArgs);
+  void (*sweepLower)(LowerArgs);
+  void (*sweepSeed)(SeedArgs);
+  void (*refine)(RefineArgs);
+  void (*lowerBoundCheck)(CheckArgs);
+};
+template <class Mask>
+CostKernels costKernelsOf() {
+  return CostKernels{sweepKernel<Mask>,      evalCostKernel<Mask>,  proposalKernel<Mask>, pingPongKernel<Mask>,
+                     sweepLowerKernel<Mask>, sweepSeedKernel<Mask>, refineKernel<Mask>,   lowerBoundCheckKernel<Mask>};
+}
+// The one place the rig size selects code: a 32-bit mask for rigs of up to 32 cameras, a 64-bit one up to 64.
+const CostKernels& costKernels(int numCams) {
+  static const CostKernels narrow = costKernelsOf<uint32_t>(), wide = costKernelsOf<uint64_t>();
+  return numCams <= kNarrowMaxCams ? narrow : wide;
+}
+
+// The most dynamic shared memory an H100 grants one CTA.
+constexpr size_t kMaxDynSmem = 227 * 1024;
+
 }  // namespace
 
 struct DerpCtx {
@@ -157,6 +182,7 @@ struct DerpCtx {
   cudaStream_t stream = nullptr;
   bool ownStream = false;
   int S = 0, Sd = 0;
+  CostKernels k{};  // costKernels(S)
   std::vector<int> dst2src;
   std::vector<DevCamera> camsNorm;  // normalised (Camera::normalizeRig)
   DevBuf<DevCamera> dCams, dCamsPx;
@@ -249,6 +275,12 @@ struct DerpCtx {
   size_t patchSmem(int threads = kPatchThreads) const {
     return (size_t)S * sizeof(DevCamera) + (size_t)2 * 9 * threads * 2 * sizeof(float) + (size_t)selSlots() * threads * sizeof(float2);
   }
+  // CTA height of the dense sweep: the tallest up to `rows` whose shared memory fits (`rows` itself up to 42 cameras;
+  // the 63 slots per thread of a 64-camera rig leave room for 12 rows)
+  int sweepRows(int rows) const {
+    while (rows > 1 && camSmem(kBlockX * rows) > kMaxDynSmem) --rows;
+    return rows;
+  }
 };
 
 namespace {
@@ -277,6 +309,19 @@ int launchCheck(DerpCtx* c, const char* what) {
   do {                                      \
     int rc_ = launchCheck(c, what);         \
     if (rc_) return rc_;                    \
+  } while (0)
+
+// A cost kernel's dynamic shared memory (cameras, tile or patches, selection slots) grows with the rig: refuse a
+// launch that would not fit instead of letting it fail.
+int checkSmem(size_t bytes, const char* what) {
+  if (bytes <= kMaxDynSmem) return DERP_OK;
+  return fail(DERP_EINVAL, std::string(what) + ": needs " + std::to_string(bytes) + " B of shared memory per CTA, more than the " +
+                               std::to_string(kMaxDynSmem) + " B an H100 grants");
+}
+#define SMEM_FITS(bytes, what)                \
+  do {                                        \
+    int rc_ = checkSmem(bytes, what);         \
+    if (rc_) return rc_;                      \
   } while (0)
 
 int resetCounters(DerpCtx* c) {
@@ -328,10 +373,11 @@ int derp_create(const DerpCameraDesc* cams, int num_cams, const int32_t* dst_to_
                 DerpCtx** out) {
   if (!cams || !dst_to_src || !out || num_cams <= 0 || num_dsts <= 0)
     return fail(DERP_EINVAL, "derp_create: bad arguments");
-  if (num_cams > kMaxCams) return fail(DERP_EINVAL, "derp_create: at most 32 cameras are supported");
+  if (num_cams > kMaxCams) return fail(DERP_EINVAL, "derp_create: at most 64 cameras are supported");
   std::unique_ptr<DerpCtx> c(new DerpCtx);
   c->device = device;
   c->S = num_cams;
+  c->k = costKernels(num_cams);
   c->Sd = num_dsts;
   c->camsNorm.resize(num_cams);
   for (int i = 0; i < num_cams; ++i) {
@@ -371,17 +417,17 @@ int derp_create(const DerpCameraDesc* cams, int num_cams, const int32_t* dst_to_
   }
 #endif
   // the cost kernels keep cameras, the destination patch tile / per-thread patches and the selection slots in
-  // dynamic shared memory: 92 KB for a 640-thread sweep CTA of a 16-camera rig, 177 KB with 32 cameras; 227 KB is
-  // the most an H100 grants one CTA
-  const int kMaxDynSmem = 227 * 1024;
-  CU(cudaFuncSetAttribute(sweepKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(evalCostKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(proposalKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(pingPongKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(sweepLowerKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(sweepSeedKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(refineKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-  CU(cudaFuncSetAttribute(lowerBoundCheckKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  // dynamic shared memory: 92 KB for a 640-thread sweep CTA of a 16-camera rig, 177 KB with 32 cameras, 216 KB for a
+  // 384-thread one with 64 cameras (DerpCtx::sweepRows); kMaxDynSmem is the most an H100 grants one CTA
+  const int maxSmem = (int)kMaxDynSmem;
+  CU(cudaFuncSetAttribute(c->k.sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.evalCost, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.proposal, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.pingPong, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.sweepLower, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.sweepSeed, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.refine, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  CU(cudaFuncSetAttribute(c->k.lowerBoundCheck, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
   *out = c.release();
   return DERP_OK;
 }
@@ -650,8 +696,9 @@ int derp_eval_cost(DerpCtx* c, int dst, const float* disparity, float* out_cost,
   CU(cudaMemcpyAsync(c->dScratchA.p, disparity, n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   if ((rc = resetCounters(c))) return rc;
   if ((rc = ensureTablesF32(c))) return rc;
-  evalCostKernel<<<grid2(c->W, c->H), block2(), c->camSmem(), c->stream>>>(c->view(dst), c->dScratchA.p, c->dScratchB.p,
-                                                                          c->dScratchC.p, c->dCounters.p);
+  SMEM_FITS(c->camSmem(), "evalCostKernel");
+  c->k.evalCost<<<grid2(c->W, c->H), block2(), c->camSmem(), c->stream>>>(c->view(dst), c->dScratchA.p, c->dScratchB.p,
+                                                                         c->dScratchC.p, c->dCounters.p);
   LAUNCHED("evalCostKernel");
   if (out_cost) CU(cudaMemcpyAsync(out_cost, c->dScratchB.p, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   if (out_conf) CU(cudaMemcpyAsync(out_conf, c->dScratchC.p, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
@@ -662,6 +709,7 @@ int derp_eval_cost(DerpCtx* c, int dst, const float* disparity, float* out_cost,
 
 #ifdef DERP_CONE_PARAMS
 static void fillCone(const DerpCtx* c, ConeCam* cone) {
+  if (c->S > kNarrowMaxCams) return;  // the wide sweepLowerKernel reads the cone fields from shared memory
   for (int s = 0; s < c->S; ++s) {
     const DevCamera& d = c->camsNorm[s];
     for (int k = 0; k < 3; ++k) {
@@ -711,13 +759,17 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
   // candidate chunks: enough CTAs to fill every SM with 8 resident CTAs even on the coarse levels
   // CTA height of the sweep: DERP_SWEEP_MAXBY rows (one 640-thread CTA per SM, 96 registers) on large levels —
   // its warps share more texel rows — and half of that (two CTAs per SM, same 20 warps) on small ones, where CTA count matters
-  // more.  DERP_SWEEP_BY overrides for tuning runs.
+  // more.  DERP_SWEEP_BY overrides for tuning runs.  Rigs of more than 42 cameras get shorter CTAs (sweepRows).
   static const int sweepBYenv = [] {
     const char* e = getenv("DERP_SWEEP_BY");
     const int v = e ? atoi(e) : 0;
     return (v >= 1 && v <= DERP_SWEEP_MAXBY) ? v : 0;
   }();
-  const int sweepBY = sweepBYenv ? sweepBYenv : (H >= 1024 ? DERP_SWEEP_MAXBY : DERP_SWEEP_MAXBY / 2);
+  const int sweepBY = c->sweepRows(sweepBYenv ? sweepBYenv : (H >= 1024 ? DERP_SWEEP_MAXBY : DERP_SWEEP_MAXBY / 2));
+  const size_t sweepSmem = c->camSmem(kBlockX * sweepBY);
+  SMEM_FITS(sweepSmem, "sweepKernel");
+  SMEM_FITS(c->camSmem(), "sweepSeedKernel");
+  SMEM_FITS(c->patchSmem(), "refineKernel");
   const dim3 g = grid2(W, H);
   const dim3 gs((W + kBlockX - 1) / kBlockX, (H + sweepBY - 1) / sweepBY, 1);
   const long ctas = (long)gs.x * gs.y * std::max(1, sweepBY / 8);
@@ -781,7 +833,7 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
 #ifdef DERP_CONE_PARAMS
     fillCone(c, la.cone);
 #endif
-    sweepLowerKernel<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), c->camSmem(kBlockX * sweepBY), c->stream>>>(la);
+    c->k.sweepLower<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), sweepSmem, c->stream>>>(la);
     LAUNCHED("sweepLowerKernel");
     SeedArgs sa;
     sa.v = a.v;
@@ -790,7 +842,7 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
     sa.disparities = a.disparities;
     sa.seed = c->dSeed.p;
     sa.best = c->dBest.p;
-    sweepSeedKernel<<<g, block2(), c->camSmem(), c->stream>>>(sa);
+    c->k.sweepSeed<<<g, block2(), c->camSmem(), c->stream>>>(sa);
     LAUNCHED("sweepSeedKernel");
     ListArgs li;
     li.W = W;
@@ -825,13 +877,13 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
         ra.list = c->dRefList.p;
         ra.count = count;
         ra.best = c->dBest.p;
-        refineKernel<<<(unsigned)((count + kPatchThreads - 1) / kPatchThreads), kPatchThreads, c->patchSmem(), c->stream>>>(ra);
+        c->k.refine<<<(unsigned)((count + kPatchThreads - 1) / kPatchThreads), kPatchThreads, c->patchSmem(), c->stream>>>(ra);
         LAUNCHED("refineKernel");
       }
     }
   }
   if (!filtered) {
-    sweepKernel<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), c->camSmem(kBlockX * sweepBY), c->stream>>>(a);
+    c->k.sweep<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), sweepSmem, c->stream>>>(a);
     LAUNCHED("sweepKernel");
   }
   if (c->profiling) {
@@ -896,7 +948,8 @@ int derp_random_proposals(DerpCtx* c, int dst, int num_proposals, float min_dept
     backgroundFillKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, a.fov, a.fg, a.bg, a.disp);
     LAUNCHED("backgroundFillKernel");
   }
-  proposalKernel<<<listGrid(W, H), kPatchThreads, c->patchSmem(), c->stream>>>(a);
+  SMEM_FITS(c->patchSmem(), "proposalKernel");
+  c->k.proposal<<<listGrid(W, H), kPatchThreads, c->patchSmem(), c->stream>>>(a);
   LAUNCHED("proposalKernel");
   return DERP_OK;
 }
@@ -922,6 +975,7 @@ int derp_ping_pong(DerpCtx* c, int dst, int iterations) {
   LAUNCHED("fillKernel");
   uint8_t* chIn = c->dChangedA.p;
   uint8_t* chOut = c->dChangedB.p;
+  SMEM_FITS(c->patchSmem(kPingThreads), "pingPongKernel");
   for (int it = 1; it <= iterations; ++it) {
     pingPongInitKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, fov, fg, bg, disp, c->dScratchA.p, c->dScratchB.p, chOut);
     LAUNCHED("pingPongInitKernel");
@@ -945,7 +999,7 @@ int derp_ping_pong(DerpCtx* c, int dst, int iterations) {
       CU(cudaEventCreate(&p1));
       CU(cudaEventRecord(p0, c->stream));
     }
-    pingPongKernel<<<listGrid(W, H, kPingThreads), kPingThreads, c->patchSmem(kPingThreads), c->stream>>>(a);
+    c->k.pingPong<<<listGrid(W, H, kPingThreads), kPingThreads, c->patchSmem(kPingThreads), c->stream>>>(a);
     LAUNCHED("pingPongKernel");
     if (c->profiling) {
       CU(cudaEventRecord(p1, c->stream));
@@ -1857,7 +1911,9 @@ int derp_debug_lower_bound(DerpCtx* c, int dst, int num_depths, float min_depth_
   fillCone(c, la.cone);
 #endif
   const int by = kBlockY;
-  sweepLowerKernel<<<dim3((W + kBlockX - 1) / kBlockX, (H + by - 1) / by, 1), dim3(kBlockX, by, 1), c->camSmem(kBlockX * by), c->stream>>>(la);
+  SMEM_FITS(c->camSmem(kBlockX * by), "sweepLowerKernel");
+  SMEM_FITS(c->camSmem(), "lowerBoundCheckKernel");
+  c->k.sweepLower<<<dim3((W + kBlockX - 1) / kBlockX, (H + by - 1) / by, 1), dim3(kBlockX, by, 1), c->camSmem(kBlockX * by), c->stream>>>(la);
   LAUNCHED("sweepLowerKernel");
   CheckArgs ca;
   ca.v = la.v;
@@ -1868,7 +1924,7 @@ int derp_debug_lower_bound(DerpCtx* c, int dst, int num_depths, float min_depth_
   ca.D = num_depths;
   ca.lb = c->dLb.p;
   ca.stats = dStats.p;
-  lowerBoundCheckKernel<<<grid2(W, H), block2(), c->camSmem(), c->stream>>>(ca);
+  c->k.lowerBoundCheck<<<grid2(W, H), block2(), c->camSmem(), c->stream>>>(ca);
   LAUNCHED("lowerBoundCheckKernel");
   unsigned long long h[5];
   CU(cudaMemcpyAsync(h, dStats.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));

@@ -29,7 +29,11 @@
 
 namespace derp {
 
-constexpr int kMaxCams = 32;                         // per-thread SSD arrays are sized by this
+// Rig size limit: evalCost's visibility mask is one machine word, 32 bits (uint32_t) for rigs of up to kNarrowMaxCams
+// cameras and 64 bits (uint64_t) above; every kernel that evaluates costs is instantiated for both (costKernels in
+// derp_b200.cu picks one per rig).
+constexpr int kMaxCams = 64;
+constexpr int kNarrowMaxCams = 32;
 constexpr float kMinVarF = 1.0f / 12.0f / 65025.0f;  // DerpUtil.h:32
 
 // One (frame, level, destination) as the cost function sees it.
@@ -633,8 +637,13 @@ __device__ __forceinline__ float lowerBoundOfCost(const V& slots, int n, int kee
   return ((kept * scaleFactor) / k) * (1.0f / k) / conf * 0.9999847412109375f;  // 1 - 2^-16
 }
 
+// Index of the lowest set bit of a non-zero visibility mask.
+__device__ __forceinline__ int lowestSetBit(uint32_t m) { return __ffs(m) - 1; }
+__device__ __forceinline__ int lowestSetBit(uint64_t m) { return __ffsll(m) - 1; }
+
 // computeCost (Derp.cpp:104-226).  `cams` points to shared memory.  Returns the cost; confidence is
 // ps.conf when the return value is not FLT_MAX, 0 otherwise.
+// Mask: the visibility mask's type, one bit per camera: uint32_t for rigs of up to 32 cameras, uint64_t up to 64.
 //
 // Structure (instruction-issue bound kernel):
 //   phase A  cone test of every source -> bitmask (short independent fp64 chains, unrolled);
@@ -652,7 +661,7 @@ __device__ __forceinline__ float lowerBoundOfCost(const V& slots, int n, int kee
 // LOWER = true: the LOWER-BOUND pass of the filtered sweep (derp_refine.cuh).  Visibility, projection, warp fetch and
 // sample positions are the exact path's; only the SSD arithmetic is replaced by a cheap approximation with a proven
 // error bound, and the return value is a number that is <= the exact cost (0 = "unknown", FLT_MAX = no source).
-template <int RP, int CP, class TX = float4, bool LOWER = false>
+template <class Mask, int RP, int CP, class TX = float4, bool LOWER = false>
 __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __restrict__ cams,
                                           const PixelState& ps, float disparity, unsigned* hits,
                                           const ConeCam* __restrict__ cone = nullptr) {
@@ -666,7 +675,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
   const float one = v.one, b23 = v.b23;
   const f32x2 one2 = pk(one, one), b232 = pk(b23, b23), half2 = pk(0.5f, 0.5f);
 
-  unsigned mask = 0;
+  Mask mask = 0;
   {
     const float fx = (float)wx, fy = (float)wy, fz = (float)wz;
     const float wL1 = fabsf(fx) + fabsf(fy) + fabsf(fz);
@@ -684,10 +693,10 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
       const int cls = -1;
 #endif
       const bool in = cls < 0 ? (cone ? insideCone(cone[s], wx, wy, wz) : insideCone(cams[s], wx, wy, wz)) : (cls != 0);
-      if (in) mask |= 1u << s;
+      if (in) mask |= Mask(1) << s;
     }
   }
-  mask &= ~(1u << v.self);
+  mask &= ~(Mask(1) << v.self);
 
   // (biased, unbiased) SSD of every contributing source: this thread's column of the [slot][thread] array in shared
   // memory, S - 1 slots (sized at launch), so no evaluation ever touches local memory.
@@ -727,11 +736,11 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
 #define DERP_PROJECT(cam) projectToSource(cam, wx, wy, wz, W, H)
 #endif
   if (mask) {
-    int s = __ffs(mask) - 1;
+    int s = lowestSetBit(mask);
     mask &= mask - 1;
     SrcPoint cur = DERP_PROJECT(cams[s]);
     while (true) {
-      const int sNext = mask ? __ffs(mask) - 1 : s;  // tail: harmless re-projection of the same source
+      const int sNext = mask ? lowestSetBit(mask) : s;  // tail: harmless re-projection of the same source
       const bool more = mask != 0;
       mask &= mask - 1;
       // ---- current source: warp entry ---------------------------------------------------------------------

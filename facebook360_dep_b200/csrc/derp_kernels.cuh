@@ -355,10 +355,12 @@ struct SweepArgs {
 
 // Launched with 32 x BY threads: BY = DERP_SWEEP_MAXBY (20 => one 640-thread CTA per SM at 96 registers) on levels of
 // >= 1024 rows, 8 on smaller ones; a taller CTA shares more texel rows between its warps (per-warp footprint (BY+3)/BY
-// rows instead of 11/8).
+// rows instead of 11/8).  Rigs of more than 42 cameras get shorter CTAs, whose S - 1 selection slots per thread still fit
+// in shared memory (DerpCtx::sweepRows).
 #ifndef DERP_SWEEP_CTAS
 #define DERP_SWEEP_CTAS 1
 #endif
+template <class Mask>
 __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepKernel(const SweepArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -383,9 +385,9 @@ __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepK
         const float d = __ldg(a.disparities + c);
         if (a.bg && !(bgd < d)) continue;  // closerMask (Derp.cpp:240-243)
 #ifdef DERP_SWEEP_U16  // measurement variant: the dense sweep on the 8-byte u16 tables
-        const float cost = evalCost<kTileW, 1, uint2>(a.v, cams, ps, d, &hits);
+        const float cost = evalCost<Mask, kTileW, 1, uint2>(a.v, cams, ps, d, &hits);
 #else
-        const float cost = evalCost<kTileW, 1>(a.v, cams, ps, d, &hits);
+        const float cost = evalCost<Mask, kTileW, 1>(a.v, cams, ps, d, &hits);
 #endif
         ++evals;
         if (cost < bestCost) {
@@ -472,6 +474,7 @@ __global__ void extendBorderKernel(int W, int H, const uint8_t* __restrict__ fg,
 }
 
 // ---- derp_eval_cost: one hypothesis per pixel ------------------------------------------------------
+template <class Mask>
 __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB)
     evalCostKernel(const CostView v, const float* __restrict__ disparity, float* __restrict__ outCost,
                    float* __restrict__ outConf, unsigned long long* counters) {
@@ -488,7 +491,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB)
     PixelState ps;
     loadPixelState(v, cams[v.self], tile, x, y, ps);
     unsigned hits = 0;
-    co = evalCost<kTileW, 1>(v, cams, ps, disparity[p], &hits);
+    co = evalCost<Mask, kTileW, 1>(v, cams, ps, disparity[p], &hits);
     cf = (co == FLT_MAX) ? 0.f : ps.conf;
     addCounters(counters, 1u, hits);
   }
@@ -613,6 +616,7 @@ __global__ void backgroundFillKernel(int W, int H, const uint8_t* __restrict__ f
   if (fov[p] && !fg[p]) disp[p] = bg[p];
 }
 
+template <class Mask>
 __global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) proposalKernel(const ProposalArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -629,7 +633,7 @@ __global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) proposalKernel
   PixelState ps;
   loadPixelStateCompact<kPatchThreads>(a.v, cams[a.v.self], patches, x, y, ps);
   float currDisp = a.disp[p];
-  float currCost = evalCost<kPatchRP, kPatchCP, uint2>(a.v, cams, ps, currDisp, &hits);
+  float currCost = evalCost<Mask, kPatchRP, kPatchCP, uint2>(a.v, cams, ps, currDisp, &hits);
   float currConf = (currCost == FLT_MAX) ? 0.f : ps.conf;
   const float costThresh = fminf(0.5f * currCost, 5.0f);
   const float minDisp = a.bg ? a.bg[p] : a.minDispGlobal;
@@ -643,7 +647,7 @@ __global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) proposalKernel
     const float lo = fmaxf(minDisp, currDisp - amplitude);
     const float hi = fminf(maxDisp, currDisp + amplitude);
     const float propDisp = rng.uniform(lo, hi);
-    const float propCost = evalCost<kPatchRP, kPatchCP, uint2>(a.v, cams, ps, propDisp, &hits);
+    const float propCost = evalCost<Mask, kPatchRP, kPatchCP, uint2>(a.v, cams, ps, propDisp, &hits);
     if (propCost < currCost && propCost < costThresh) {
       currCost = propCost;
       currDisp = propDisp;
@@ -693,6 +697,7 @@ __global__ void pingPongInitKernel(int W, int H, const uint8_t* __restrict__ fov
   changedNext[p] = (old != res) ? 1 : 0;
 }
 
+template <class Mask>
 __global__ void __launch_bounds__(kPingThreads, DERP_PING_MINB) pingPongKernel(const PingPongArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -722,7 +727,7 @@ __global__ void __launch_bounds__(kPingThreads, DERP_PING_MINB) pingPongKernel(c
     if (!a.fov[q]) continue;
     const float d = a.disp[q];
     if (d >= backgroundDisparity && a.changed[q]) {
-      const float cost = evalCost<3 * kPingThreads, kPingThreads, uint2>(a.v, cams, ps, d, &hits);
+      const float cost = evalCost<Mask, 3 * kPingThreads, kPingThreads, uint2>(a.v, cams, ps, d, &hits);
       ++evals;
       if (cost < bestCost) {
         bestCost = cost;
@@ -767,7 +772,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) mismatchKernel(const Mismatc
   }
   const float dispCurr = a.dispAll[a.self * plane + p];
   int nMatch = 0, nMis = 0;
-  float mis[kMaxCams];
+  float mis[kMaxCams];  // disparities of the disagreeing sources: at most S - 1 of them
   if (!a.fg || a.fg[p]) {
     const DevCamera& cd = cams[a.self];
     double dir[3];

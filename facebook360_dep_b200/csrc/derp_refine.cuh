@@ -32,10 +32,11 @@ struct LowerArgs {
   unsigned long long* seed;    // [H][W]  (L bits << 32 | candidate), atomicMin across candidate chunks
   unsigned long long* counters;
 #ifdef DERP_CONE_PARAMS
-  ConeCam cone[kMaxCams];      // cone-test fields of every camera, read from the constant bank (derp_cost.cuh)
+  ConeCam cone[kNarrowMaxCams];  // cone-test fields of every camera, read from the constant bank (derp_cost.cuh)
 #endif
 };
 
+template <class Mask>
 __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepLowerKernel(const LowerArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -62,9 +63,10 @@ __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepL
         float L = FLT_MAX;
         if (!(a.bg && !(bgd < d))) {  // closerMask (Derp.cpp:240-243)
 #ifdef DERP_CONE_PARAMS
-          L = evalCost<kTileW, 1, float4, true>(a.v, cams, ps, d, &hits, a.cone);
+          // the parameter block holds kNarrowMaxCams cameras: wider rigs read the cone fields from shared memory
+          L = evalCost<Mask, kTileW, 1, float4, true>(a.v, cams, ps, d, &hits, sizeof(Mask) == 4 ? a.cone : nullptr);
 #else
-          L = evalCost<kTileW, 1, float4, true>(a.v, cams, ps, d, &hits);
+          L = evalCost<Mask, kTileW, 1, float4, true>(a.v, cams, ps, d, &hits);
 #endif
           ++evals;
         }
@@ -94,6 +96,7 @@ struct SeedArgs {
 };
 
 // exact cost of the seed candidate; same CTA shape and shared-memory layout as evalCostKernel
+template <class Mask>
 __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) sweepSeedKernel(const SeedArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -110,7 +113,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) sweepSeedKe
   PixelState ps;
   loadPixelState(a.v, cams[a.v.self], tile, x, y, ps);
   unsigned hits = 0;
-  const float cost = evalCost<kTileW, 1>(a.v, cams, ps, __ldg(a.disparities + cstar), &hits);
+  const float cost = evalCost<Mask, kTileW, 1>(a.v, cams, ps, __ldg(a.disparities + cstar), &hits);
   if (cost < FLT_MAX) a.best[p] = ((unsigned long long)__float_as_uint(cost) << 32) | (unsigned long long)cstar;
 }
 
@@ -167,6 +170,7 @@ struct RefineArgs {
   unsigned long long* best;
 };
 
+template <class Mask>
 __global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) refineKernel(const RefineArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -180,7 +184,7 @@ __global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) refineKernel(c
   PixelState ps;
   loadPixelStateCompactF32(a.v, cams[a.v.self], patches, x, y, ps);
   unsigned hits = 0;
-  const float cost = evalCost<kPatchRP, kPatchCP, float4>(a.v, cams, ps, __ldg(a.disparities + c), &hits);
+  const float cost = evalCost<Mask, kPatchRP, kPatchCP, float4>(a.v, cams, ps, __ldg(a.disparities + c), &hits);
   if (cost < FLT_MAX) atomicMin(a.best + p, ((unsigned long long)__float_as_uint(cost) << 32) | (unsigned long long)c);
 }
 
@@ -198,6 +202,7 @@ struct CheckArgs {
   unsigned long long* stats;
 };
 
+template <class Mask>
 __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) lowerBoundCheckKernel(const CheckArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
@@ -225,7 +230,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) lowerBoundC
         continue;
       }
       unsigned hits = 0;
-      const float cost = evalCost<kTileW, 1>(a.v, cams, ps, d, &hits);
+      const float cost = evalCost<Mask, kTileW, 1>(a.v, cams, ps, d, &hits);
       ++n;
       if (L > cost) ++bad;
       if (L == 0.0f) ++unk;

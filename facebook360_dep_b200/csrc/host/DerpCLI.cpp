@@ -370,7 +370,8 @@ int main(int argc, char* argv[]) {
   Shared sh;
   sh.rig = io::loadRig(FLAGS_rig);
   CHECK_GT(sh.rig.cams.size(), 0u) << "no source cameras!";
-  CHECK_LE(sh.rig.cams.size(), 32u) << "this build handles rigs of up to 32 cameras (source-visibility masks are 32-bit); the "
+  // checked before any sharding, so it covers every --gpus layout
+  CHECK_LE(sh.rig.cams.size(), 64u) << "this build handles rigs of up to 64 cameras (source-visibility masks are 64-bit); the "
                                        "reference has no such limit";
   sh.dst = io::filterDestinations(sh.rig, FLAGS_cameras);
   CHECK_GT(sh.dst.size(), 0u) << "no destination cameras!";
