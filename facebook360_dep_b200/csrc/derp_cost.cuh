@@ -740,7 +740,10 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
     mask &= mask - 1;
     SrcPoint cur = DERP_PROJECT(cams[s]);
     while (true) {
-      const int sNext = mask ? lowestSetBit(mask) : s;  // tail: harmless re-projection of the same source
+      // Tail (!more): the exact path re-projects the same source, harmlessly, to keep its main block straight-line
+      // code.  The lower-bound pass skips that projection: in a warp's last iteration no lane needs it, and measured
+      // on the headline sweep the branch costs less than the fp64 projection it saves.
+      const int sNext = mask ? lowestSetBit(mask) : s;
       const bool more = mask != 0;
       mask &= mask - 1;
       // ---- current source: warp entry ---------------------------------------------------------------------
@@ -782,7 +785,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
           const TX* r3 = r2 + W;
           const TX* b1 = srcBiasImg + off + W + 1;  // bias sample = centre sample's 2x2 footprint
           if constexpr (LOWER) {
-            nxt = DERP_PROJECT(cams[sNext]);
+            if (more) nxt = DERP_PROJECT(cams[sNext]);
             float sB, sU;
             ssdApprox<RP, CP>(r0, r1, r2, r3, b1, W, ps, W0, W1, W2, &sB, &sU);
             // slot = (sqrt of the biased sum, lower bound of the unbiased sum), see lowerBoundOfCost
@@ -869,7 +872,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
           pushPair(sB * scaleFactor, sU * scaleFactor);
           }
         } else {
-          nxt = projectToSource(cams[sNext], wx, wy, wz, W, H);
+          if (!LOWER || more) nxt = projectToSource(cams[sNext], wx, wy, wz, W, H);
           if constexpr (LOWER) {
             if (!(isnan(xDstSrc) || isnan(yDstSrc))) {  // the source contributes, through the generic path
               unknown = true;
@@ -883,7 +886,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
           }
         }
       } else {
-        nxt = projectToSource(cams[sNext], wx, wy, wz, W, H);
+        if (!LOWER || more) nxt = projectToSource(cams[sNext], wx, wy, wz, W, H);
       }
       if (!more) break;
       cur = nxt;
