@@ -314,6 +314,77 @@ def _ptr_array(arrs):
     return pa
 
 
+# ---- include/derp_rephoto.h ---------------------------------------------------------------------------------------
+_REPHOTO_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_rephoto_cubemap": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, _p(C.c_void_p), _p(C.c_void_p), C.c_int, C.c_int,
+                                       C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "derp_rephoto_score": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_void_p, C.c_void_p]),
+}
+REPHOTO_SYMBOLS = sorted(k for k in _REPHOTO_SIGS if k.startswith("derp_rephoto_"))
+REPHOTO_METHODS = {"MSSIM": 0, "NCC": 1}
+
+
+class Rephoto:
+    """ctypes binding of include/derp_rephoto.h on a loaded library: ``Rephoto(load_cuda())`` for the product, or a
+    path to another library exporting the same entry points (the CPU checker the tests build)."""
+
+    def __init__(self, library):
+        if isinstance(library, Library):
+            self.path, self.lib = library.path, C.CDLL(library.path, mode=C.RTLD_LOCAL)
+        else:
+            if not os.path.exists(library):
+                raise FileNotFoundError(library)
+            self.path, self.lib = library, C.CDLL(library, mode=C.RTLD_LOCAL)
+        for name, (res, args) in _REPHOTO_SIGS.items():
+            fn = getattr(self.lib, name)  # AttributeError if a declared symbol is missing
+            fn.restype = res
+            fn.argtypes = args
+
+    def _check(self, rc):
+        if rc != 0:
+            raise DerpError(rc, self.lib.derp_last_error().decode())
+
+    def rephoto_cubemap(self, descs, disparities, colors_bgra, center, edge, want_color=True, want_disparity=False,
+                        want_winners=False, device=0):
+        """CanopyScene(rig, disparities, colors).cubemap(edge, center) (ComputeRephotographyErrors.cpp:77-95): float
+        B, G, R, A cubemaps [6 * edge, edge, 4] (faces +X, -X, +Y, -Y, +Z, -Z stacked), NaN set to 0.  disparities:
+        float [h, w] per camera; colors_bgra: float [h, w, 4] per camera at the disparity's size.  Returns
+        (color, disparity, winners), each None unless asked for; winners int32 [num_cams, 6 * edge, edge]."""
+        S = len(disparities)
+        d = [np.ascontiguousarray(x, np.float32) for x in disparities]
+        h, w = d[0].shape if S else (2, 2)
+        assert all(x.shape == (h, w) for x in d)
+        cols = None
+        if want_color and S:
+            cols = [np.ascontiguousarray(x, np.float32) for x in colors_bgra]
+            assert all(x.shape == (h, w, 4) for x in cols)
+        ctr = np.ascontiguousarray(center, np.float32)
+        oc = np.empty((6 * edge, edge, 4), np.float32) if want_color else None
+        od = np.empty((6 * edge, edge, 4), np.float32) if want_disparity else None
+        wn = np.empty((max(S, 1), 6 * edge, edge), np.int32) if want_winners else None
+        dp = _ptr_array(d) if S else None
+        cp = _ptr_array(cols) if cols else None
+        self._check(self.lib.derp_rephoto_cubemap(device, descs, S, dp, cp, w, h, ctr.ctypes.data, edge, _dp(oc), _dp(od),
+                                                 _dp(wn)))
+        return oc, od, (wn[:S] if wn is not None else None)
+
+    def rephoto_score(self, ref_bgr, ren_bgr, mask, method="MSSIM", stat_radius=1, device=0):
+        """computeScoreMap + averageScore (RephotographyUtil.h:39-120): returns (score map float [h, w, 3] B, G, R,
+        per-channel averages over the mask without NaN as a float64 [3] in B, G, R order)."""
+        x = np.ascontiguousarray(ref_bgr, np.float32)
+        y = np.ascontiguousarray(ren_bgr, np.float32)
+        m = np.ascontiguousarray(mask, np.uint8)
+        h, w = x.shape[:2]
+        assert x.shape == (h, w, 3) and y.shape == (h, w, 3) and m.shape == (h, w)
+        score = np.empty((h, w, 3), np.float32)
+        avg = np.empty(3, np.float64)
+        self._check(self.lib.derp_rephoto_score(device, x.ctypes.data, y.ctypes.data, m.ctypes.data, w, h,
+                                               REPHOTO_METHODS[method], stat_radius, score.ctypes.data, avg.ctypes.data))
+        return score, avg
+
+
 class Context:
     """One DerpCtx: a (frame, level) of a rig on one device."""
 

@@ -21,6 +21,8 @@
 #include "derp_mesh.cuh"
 #include "derp_simplify.h"
 #include "derp_bc7.cuh"
+#include "derp_rephoto.cuh"
+#include "../../include/derp_rephoto.h"
 
 using namespace derp;
 
@@ -2087,6 +2089,185 @@ int derp_bc7_compress_image(int device, const void* pixels, int bits_per_channel
   derp::bc7::gammaTable(bits_per_channel, gamma, lut.data());
   return bc7Launch(device, pixels, (size_t)width * height * channels * (bits_per_channel / 8), bits_per_channel, channels,
                    width, height, lut.data(), lut.size(), blocks);
+}
+
+}  // extern "C"
+
+// ---- rephotography (derp_rephoto.cuh) ----------------------------------------------------------------
+// Grow-only scratch per host thread, like the camera mesh: the app renders four cubemaps and one score per camera.
+namespace {
+struct RephotoScratch {
+  DevBuf<float> disp, bgra, vtx, out, f32;
+  DevBuf<ushort4> texC, texD;
+  DevBuf<unsigned long long> keys;
+  DevBuf<float4> accC, accD;
+  DevBuf<int> flags;
+  DevBuf<int32_t> win;
+  DevBuf<uint8_t> mask;
+  DevBuf<double> partial;
+  int device = -1;
+  void release() {
+    disp.release(); bgra.release(); vtx.release(); out.release(); f32.release(); texC.release(); texD.release();
+    keys.release(); accC.release(); accD.release(); flags.release(); win.release(); mask.release(); partial.release();
+  }
+};
+thread_local RephotoScratch g_rephoto;
+
+int rephotoScratch(int device) {
+  RephotoScratch& s = g_rephoto;
+  if (s.device != device) {
+    if (s.device >= 0) {
+      cudaSetDevice(s.device);
+      s.release();
+    }
+    s.device = device;
+  }
+  CU(cudaSetDevice(device));
+  return DERP_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int derp_rephoto_cubemap(int device, const DerpCameraDesc* cams, int num_cams, const float* const* disparities,
+                         const float* const* colors_bgra, int width, int height, const float* center, int edge,
+                         float* out_color, float* out_disparity, int32_t* winners) {
+  using namespace derp::rephoto;
+  if (!cams || num_cams < 0 || (num_cams > 0 && !disparities) || width < 2 || height < 2 || !center || edge < 2 ||
+      (!out_color && !out_disparity) || (out_color && num_cams > 0 && !colors_bgra))
+    return fail(DERP_EINVAL, "derp_rephoto_cubemap: bad arguments");
+  if ((long long)width * height >= (1ll << 30) || (long long)edge * edge * kFaces >= (1ll << 31))
+    return fail(DERP_EINVAL, "derp_rephoto_cubemap: image or cubemap too large");
+  std::vector<DevCamera> dc(num_cams);
+  for (int i = 0; i < num_cams; ++i) {
+    DevCamera c;
+    if (!host::makeCamera(cams[i], &c)) return fail(DERP_EINVAL, "derp_rephoto_cubemap: invalid camera " + std::to_string(i));
+    dc[i] = host::rescaled(c, width, height);  // camera.rescale({disparity.cols, disparity.rows})
+  }
+  int rc = rephotoScratch(device);
+  if (rc) return rc;
+  RephotoScratch& s = g_rephoto;
+  const size_t n = (size_t)width * height;
+  int levels = 1;
+  while ((width >> levels) > 0 || (height >> levels) > 0) ++levels;
+  if (levels > kMaxLevels) return fail(DERP_EINVAL, "derp_rephoto_cubemap: image too large");
+  Canopy cv{};
+  cv.w = width;
+  cv.h = height;
+  cv.levels = levels;
+  long long texels = 0;
+  for (int l = 0; l < levels; ++l) {
+    cv.lw[l] = std::max(1, width >> l);
+    cv.lh[l] = std::max(1, height >> l);
+    cv.lofs[l] = texels;
+    texels += (long long)cv.lw[l] * cv.lh[l];
+  }
+  const size_t pixels = (size_t)kFaces * edge * edge;
+  CU(s.disp.ensure(n));
+  CU(s.vtx.ensure(n * 3));
+  CU(s.keys.ensure(pixels));
+  CU(s.flags.ensure(1));
+  if (out_color) {
+    CU(s.bgra.ensure(n * 4));
+    CU(s.texC.ensure(texels));
+    CU(s.accC.ensure(pixels));
+    CU(cudaMemset(s.accC.p, 0, pixels * sizeof(float4)));
+  }
+  if (out_disparity) {
+    CU(s.texD.ensure(texels));
+    CU(s.accD.ensure(pixels));
+    CU(cudaMemset(s.accD.p, 0, pixels * sizeof(float4)));
+  }
+  if (winners) CU(s.win.ensure(pixels * std::max(num_cams, 1)));
+  CU(s.out.ensure(pixels * 4));
+  FaceMats fm;
+  faceMatrices(center, &fm);
+  cv.vtx = s.vtx.p;
+  cv.tex[0] = out_color ? s.texC.p : nullptr;
+  cv.tex[1] = out_disparity ? s.texD.p : nullptr;
+  const int prims = (width - 1) * (height - 1) * 2;
+  for (int i = 0; i < num_cams; ++i) {  // canopies in camera order: the blend sums are order-dependent
+    CU(cudaMemcpy(s.disp.p, disparities[i], n * sizeof(float), cudaMemcpyDefault));
+    if (out_color) CU(cudaMemcpy(s.bgra.p, colors_bgra[i], n * 4 * sizeof(float), cudaMemcpyDefault));
+    CU(cudaMemset(s.flags.p, 0, sizeof(int)));
+    rephotoPrepKernel<<<dim3((width + 127) / 128, height), 128>>>(dc[i], s.disp.p, s.bgra.p, width, height, center[0],
+                                                                  center[1], center[2], s.vtx.p,
+                                                                  out_color ? s.texC.p : nullptr,
+                                                                  out_disparity ? s.texD.p : nullptr, s.flags.p);
+    for (int l = 1; l < levels; ++l)
+      for (int t = 0; t < 2; ++t) {
+        ushort4* tex = t == 0 ? (out_color ? s.texC.p : nullptr) : (out_disparity ? s.texD.p : nullptr);
+        if (!tex) continue;
+        rephotoMipKernel<<<dim3((cv.lw[l] + 127) / 128, cv.lh[l]), 128>>>(tex + cv.lofs[l - 1], cv.lw[l - 1], cv.lh[l - 1],
+                                                                          tex + cv.lofs[l], cv.lw[l], cv.lh[l]);
+      }
+    CU(cudaMemcpy(&cv.anyZeroAlpha, s.flags.p, sizeof(int), cudaMemcpyDeviceToHost));
+    CU(cudaMemset(s.keys.p, 0xff, pixels * sizeof(unsigned long long)));
+    rephotoRasterKernel<<<dim3((prims + 255) / 256, kFaces), 256>>>(cv, fm, edge, prims, s.keys.p);
+    rephotoResolveKernel<<<grid1(pixels), 256>>>(cv, fm, edge, s.keys.p, out_color ? s.accC.p : nullptr,
+                                                 out_disparity ? s.accD.p : nullptr,
+                                                 winners ? s.win.p + (size_t)i * pixels : nullptr);
+    CU(cudaGetLastError());
+  }
+  for (int t = 0; t < 2; ++t) {
+    float* dst = t == 0 ? out_color : out_disparity;
+    if (!dst) continue;
+    rephotoUnpremulKernel<<<grid1(pixels), 256>>>(pixels, t == 0 ? s.accC.p : s.accD.p, s.out.p);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(dst, s.out.p, pixels * 4 * sizeof(float), cudaMemcpyDefault));
+  }
+  if (winners && num_cams > 0)
+    CU(cudaMemcpy(winners, s.win.p, pixels * num_cams * sizeof(int32_t), cudaMemcpyDefault));
+  CU(cudaDeviceSynchronize());
+  return DERP_OK;
+}
+
+int derp_rephoto_score(int device, const float* ref_bgr, const float* ren_bgr, const uint8_t* mask, int width, int height,
+                       int method, int stat_radius, float* score_map, double* avg) {
+  using namespace derp::rephoto;
+  if (!ref_bgr || !ren_bgr || !mask || width < 1 || height < 1 || !score_map || !avg)
+    return fail(DERP_EINVAL, "derp_rephoto_score: bad arguments");
+  if (method != DERP_REPHOTO_MSSIM && method != DERP_REPHOTO_NCC)
+    return fail(DERP_EINVAL, "derp_rephoto_score: method must be DERP_REPHOTO_MSSIM or DERP_REPHOTO_NCC");
+  if (stat_radius < 1 || stat_radius > 31) return fail(DERP_EINVAL, "derp_rephoto_score: stat_radius in [1, 31]");
+  int rc = rephotoScratch(device);
+  if (rc) return rc;
+  RephotoScratch& s = g_rephoto;
+  const size_t pixels = (size_t)width * height, n = pixels * 3;
+  // f32 layout: [x | y | mu (2n) | moments (3n) | sig (3n) | tmp (3n) | weights (64)]
+  CU(s.f32.ensure(13 * n + 64));
+  float *x = s.f32.p, *y = x + n, *mu = y + n, *mom = mu + 2 * n, *sig = mom + 3 * n, *tmp = sig + 3 * n,
+        *wt = tmp + 3 * n;
+  float hw[64];
+  gaussianWeights(stat_radius, hw);
+  const unsigned blocks = grid1(pixels);
+  CU(s.mask.ensure(pixels));
+  CU(s.out.ensure(n));
+  CU(s.partial.ensure((size_t)blocks * 6));
+  CU(cudaMemcpy(x, ref_bgr, n * sizeof(float), cudaMemcpyDefault));
+  CU(cudaMemcpy(y, ren_bgr, n * sizeof(float), cudaMemcpyDefault));
+  CU(cudaMemcpy(s.mask.p, mask, pixels, cudaMemcpyDefault));
+  CU(cudaMemcpy(wt, hw, (2 * stat_radius + 1) * sizeof(float), cudaMemcpyHostToDevice));
+  const dim3 g2((width + 127) / 128, height, 2), g3((width + 127) / 128, height, 3);
+  rephotoBlurRowsKernel<<<g2, 128>>>(x, width, height, stat_radius, wt, tmp);  // x, y are adjacent: two images
+  rephotoBlurColsKernel<<<g2, 128>>>(tmp, width, height, stat_radius, wt, mu);
+  rephotoMomentsKernel<<<grid1(n), 256>>>(n, x, y, mu, mom);
+  rephotoBlurRowsKernel<<<g3, 128>>>(mom, width, height, stat_radius, wt, tmp);
+  rephotoBlurColsKernel<<<g3, 128>>>(tmp, width, height, stat_radius, wt, sig);
+  rephotoScoreKernel<<<blocks, 256>>>(pixels, mu, sig, s.mask.p, method == DERP_REPHOTO_NCC, s.out.p, s.partial.p);
+  CU(cudaGetLastError());
+  std::vector<double> part((size_t)blocks * 6);
+  CU(cudaMemcpy(score_map, s.out.p, n * sizeof(float), cudaMemcpyDefault));
+  CU(cudaMemcpy(part.data(), s.partial.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  for (int c = 0; c < 3; ++c) {  // cv::mean(channel, mask without NaN): 0 for an empty mask
+    double sum = 0, cnt = 0;
+    for (unsigned b = 0; b < blocks; ++b) {
+      sum += part[b * 6 + c];
+      cnt += part[b * 6 + 3 + c];
+    }
+    avg[c] = cnt > 0 ? sum / cnt : 0.0;
+  }
+  return DERP_OK;
 }
 
 }  // extern "C"

@@ -457,7 +457,7 @@ inline void pngChunk(std::ofstream& f, const char* type, const std::vector<uint8
   f.write(reinterpret_cast<char*>(c), 4);
 }
 
-// 8-bit PNG, `channels` = 1 (gray) or 4 (BGRA input, written as RGBA) — what cv::imwrite produces for a CV_32F matrix:
+// 8-bit PNG, `channels` = 1 (gray), 3 (BGR input, written as RGB) or 4 (BGRA input, written as RGBA) — what cv::imwrite produces for a CV_32F matrix:
 // it converts to CV_8U first (convertTo, i.e. saturate_cast<uchar>(cvRound(v)); modules/imgcodecs loadsave.cpp)
 inline void writePng8(const fs::path& path, const uint8_t* data, int w, int h, int channels) {
   std::ofstream f(path, std::ios::binary);
@@ -468,7 +468,7 @@ inline void writePng8(const fs::path& path, const uint8_t* data, int w, int h, i
   ihdr[0] = w >> 24; ihdr[1] = w >> 16; ihdr[2] = w >> 8; ihdr[3] = w;
   ihdr[4] = h >> 24; ihdr[5] = h >> 16; ihdr[6] = h >> 8; ihdr[7] = h;
   ihdr[8] = 8;
-  ihdr[9] = channels == 1 ? 0 : 6;
+  ihdr[9] = channels == 1 ? 0 : channels == 3 ? 2 : 6;
   pngChunk(f, "IHDR", ihdr);
   const size_t stride = (size_t)w * channels;
   std::vector<uint8_t> raw((stride + 1) * h);
@@ -478,6 +478,12 @@ inline void writePng8(const fs::path& path, const uint8_t* data, int w, int h, i
     const uint8_t* in = data + (size_t)y * stride;
     if (channels == 1) {
       std::memcpy(out, in, stride);
+    } else if (channels == 3) {
+      for (int x = 0; x < w; ++x, in += 3, out += 3) {
+        out[0] = in[2];
+        out[1] = in[1];
+        out[2] = in[0];
+      }
     } else {
       for (int x = 0; x < w; ++x, in += 4, out += 4) {
         out[0] = in[2];
