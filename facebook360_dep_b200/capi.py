@@ -385,6 +385,83 @@ class Rephoto:
         return score, avg
 
 
+# ---- include/derp_canopy.h ----------------------------------------------------------------------------------------
+_CANOPY_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_canopy_render": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, _p(C.c_void_p), C.c_int, C.c_int, _p(C.c_void_p),
+                                     C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float,
+                                     C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+}
+CANOPY_SYMBOLS = sorted(k for k in _CANOPY_SIGS if k.startswith("derp_canopy_")) + ["derp_canopy_snapshot_matrix"]
+CANOPY_PROJECTIONS = {"cubemap": 0, "equirect": 1, "perspective": 2}
+CANOPY_SHADERS = {"on_screen": 0, "svd": 1}
+
+
+class Canopy:
+    """ctypes binding of include/derp_canopy.h's renderer on a loaded library: ``Canopy(load_cuda())`` for the product,
+    or a path to another library exporting derp_canopy_render (the CPU checker the tests build)."""
+
+    def __init__(self, library):
+        path = library.path if isinstance(library, Library) else library
+        if not os.path.exists(path):
+            raise FileNotFoundError(path)
+        self.path, self.lib = path, C.CDLL(path, mode=C.RTLD_LOCAL)
+        for name, (res, args) in _CANOPY_SIGS.items():
+            fn = getattr(self.lib, name)  # AttributeError if a declared symbol is missing
+            fn.restype = res
+            fn.argtypes = args
+
+    def _check(self, rc):
+        if rc != 0:
+            raise DerpError(rc, self.lib.derp_last_error().decode())
+
+    def render(self, descs, disparities, colors_bgra, position, projection="cubemap", size=(64, 64), matrix=None,
+               ipd=0.0, alpha_blend=True, shader="svd", want_color=True, want_disparity=False, want_winners=False,
+               device=0):
+        """CanopyScene(rig, disparities, colors).cubemap / equirect / render from `position` (derp_canopy.h).
+        disparities: float [h, w] per camera (the mesh); colors_bgra: float [ch, cw, 4] per camera at any one size.
+        size = (out_width, out_height): (edge, edge) for the cubemap, (2 h, h) for the equirect.  Returns (color,
+        disparity, winners), each None unless asked for: float B, G, R, A images with NaN where nothing covers, winners
+        int32 [num_cams, raster rows, raster width]."""
+        S = len(disparities)
+        d = [np.ascontiguousarray(x, np.float32) for x in disparities]
+        h, w = d[0].shape if S else (2, 2)
+        assert all(x.shape == (h, w) for x in d)
+        cols, ch, cw = None, 0, 0
+        if want_color:
+            cols = [np.ascontiguousarray(x, np.float32) for x in colors_bgra]
+            ch, cw = cols[0].shape[:2] if S else (1, 1)
+            assert all(x.shape == (ch, cw, 4) for x in cols)
+        proj = CANOPY_PROJECTIONS[projection]
+        W, H = size
+        shape = {0: (6 * H, W), 1: (H, 2 * H), 2: (H, W)}[proj]
+        raster = (6 * H, H) if proj != 2 else (H, W)
+        pos = np.ascontiguousarray(position, np.float32)
+        m = None if matrix is None else np.ascontiguousarray(matrix, np.float32).reshape(16)
+        oc = np.empty(shape + (4,), np.float32) if want_color else None
+        od = np.empty(shape + (4,), np.float32) if want_disparity else None
+        wn = np.empty((max(S, 1),) + raster, np.int32) if want_winners else None
+        self._check(self.lib.derp_canopy_render(device, descs, S, _ptr_array(d) if S else None, w, h,
+                                                _ptr_array(cols) if cols else None, cw, ch, proj, pos.ctypes.data,
+                                                _dp(m), W, H, float(ipd), int(bool(alpha_blend)), CANOPY_SHADERS[shader],
+                                                _dp(oc), _dp(od), _dp(wn)))
+        return oc, od, (wn[:S] if wn is not None else None)
+
+
+def snapshot_matrix(position, forward, up, horizontal_fov=90.0, width=3072, height=1536, library=None):
+    """SimpleMeshRenderer's snapshot clip matrix (derp_canopy_snapshot_matrix, computed on the host): float32 [4, 4]."""
+    lib = library.lib if library is not None else load_cuda().lib
+    f = lib.derp_canopy_snapshot_matrix
+    f.restype = C.c_int
+    f.argtypes = [C.c_void_p] * 3 + [C.c_double, C.c_int, C.c_int, C.c_void_p]
+    vec = [np.ascontiguousarray(v, np.float32) for v in (position, forward, up)]
+    out = np.empty(16, np.float32)
+    rc = f(vec[0].ctypes.data, vec[1].ctypes.data, vec[2].ctypes.data, horizontal_fov, width, height, out.ctypes.data)
+    if rc != 0:
+        raise DerpError(rc, lib.derp_last_error().decode())
+    return out.reshape(4, 4)
+
+
 class Context:
     """One DerpCtx: a (frame, level) of a rig on one device."""
 

@@ -39,39 +39,11 @@ DEFINE_int32(gpu, 0, "CUDA device to use");
     if (rc_ != 0) LOG(FATAL) << #expr << " failed: " << derp_last_error(); \
   } while (0)
 
-// cv_util::loadImage<cv::Vec4f>: integer samples * (1 / max), alpha 1 when the file has none
-static std::vector<float> loadColorF32x4(const fs::path& p, int* w, int* h) {
-  const io::Image img = io::loadUnchanged(p);
-  *w = img.w;
-  *h = img.h;
-  const size_t n = (size_t)img.w * img.h;
-  std::vector<float> out(n * 4);
-  const float scale = img.bits == 16 ? 1.0f / 65535.0f : 1.0f / 255.0f;
-  for (size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 4; ++c) {
-      float v = 1.0f;
-      if (c < 3 || img.channels == 4) {
-        const size_t idx = i * img.channels + (img.channels >= 3 ? c : 0);
-        v = img.bits == 32 ? img.f[idx] : img.u[idx] * scale;
-      }
-      out[i * 4 + c] = v;
-    }
-  return out;
-}
-
 // rephoto_util::formatResults: R, G, B from a B, G, R scalar
 static std::string formatResults(const double* s) {
   char buf[128];
   std::snprintf(buf, sizeof(buf), "R %.2f%%, G %.2f%%, B %.2f%%", 100 * s[2], 100 * s[1], 100 * s[0]);
   return buf;
-}
-
-static void verifyImagePaths(const std::string& dir, const io::Rig& rig, int first, int last, const std::string& ext) {
-  for (const std::string& id : rig.ids)
-    for (int f = first; f <= last; ++f) {
-      const fs::path p = ext.empty() ? io::imagePath(dir, id, io::zeroPad(f)) : fs::path(dir) / id / (io::zeroPad(f) + ext);
-      CHECK(fs::exists(p)) << "missing file: " << p.string();
-    }
 }
 
 int main(int argc, char** argv) {
@@ -89,8 +61,8 @@ int main(int argc, char** argv) {
   const int S = (int)rig.cams.size();
   CHECK_GT(S, 0);
   const int first = std::stoi(FLAGS_first), last = std::stoi(FLAGS_last);
-  verifyImagePaths(FLAGS_color, rig, first, last, "");
-  verifyImagePaths(FLAGS_disparity, rig, first, last, ".pfm");
+  io::verifyImagePaths(FLAGS_color, rig, first, last, "");
+  io::verifyImagePaths(FLAGS_disparity, rig, first, last, ".pfm");
   LOG(INFO) << "backend " << derp_backend();
 
   const fs::path rephotoDir = fs::path(FLAGS_output) / "rephoto";
@@ -122,7 +94,7 @@ int main(int argc, char** argv) {
     }
     for (int i = 0; i < S; ++i) {  // loadResizedImages<Vec4f>(..., disps[0].size(), INTER_AREA)
       int w, h;
-      std::vector<float> c = loadColorF32x4(io::imagePath(FLAGS_color, rig.ids[i], frameName), &w, &h);
+      std::vector<float> c = io::loadColorF32x4(io::imagePath(FLAGS_color, rig.ids[i], frameName), &w, &h);
       if (w != W || h != H) {
         std::vector<float> r((size_t)W * H * 4);
         io::area::resize(c.data(), w, h, 4, r.data(), W, H);

@@ -509,9 +509,10 @@ inline uint8_t saturateU8(float v) {
   return (uint8_t)(r < 0 ? 0 : r > 255 ? 255 : r);
 }
 
-// One-channel 32-bit float OpenEXR file (scan lines, no compression, channel "Y" like OpenCV's grayscale EXR output):
-// the layout of the OpenEXR file-format document — magic, version, attribute list, line offset table, scan lines.
-inline void writeExrFloat(const fs::path& path, const float* data, int w, int h) {
+// 32-bit float OpenEXR file (scan lines, no compression) of 1 channel ("Y", like OpenCV's grayscale EXR output) or 3
+// interleaved B, G, R channels (channels "B", "G", "R", as OpenCV names them): the layout of the OpenEXR file-format
+// document — magic, version, attribute list, line offset table, scan lines holding each channel's row in chlist order.
+inline void writeExrFloatChannels(const fs::path& path, const float* data, int w, int h, int channels) {
   std::ofstream f(path, std::ios::binary);
   CHECK(f.good()) << "failed to save image: " << path.string();
   std::vector<uint8_t> hd;
@@ -535,13 +536,17 @@ inline void writeExrFloat(const fs::path& path, const float* data, int w, int h)
   };
   put32(hd, 20000630u);  // magic
   put32(hd, 2u);         // version 2, single-part scan-line file
+  CHECK(channels == 1 || channels == 3) << "EXR output of 1 or 3 channels";
+  static const char* names3[3] = {"B", "G", "R"};  // chlist order (alphabetical); B is interleaved channel 0
   {
     std::vector<uint8_t> v;
-    putS(v, "Y");
-    put32(v, 2);  // FLOAT
-    put32(v, 0);  // pLinear + reserved
-    put32(v, 1);  // xSampling
-    put32(v, 1);  // ySampling
+    for (int c = 0; c < channels; ++c) {
+      putS(v, channels == 1 ? "Y" : names3[c]);
+      put32(v, 2);  // FLOAT
+      put32(v, 0);  // pLinear + reserved
+      put32(v, 1);  // xSampling
+      put32(v, 1);  // ySampling
+    }
     v.push_back(0);
     attr("channels", "chlist", v);
   }
@@ -574,22 +579,27 @@ inline void writeExrFloat(const fs::path& path, const float* data, int w, int h)
   }
   hd.push_back(0);  // end of header
   f.write(reinterpret_cast<const char*>(hd.data()), (std::streamsize)hd.size());
-  const uint64_t lineBytes = 8 + (uint64_t)w * 4;
+  const uint64_t lineBytes = 8 + (uint64_t)w * 4 * channels;
   uint64_t ofs = hd.size() + (uint64_t)h * 8;
   for (int y = 0; y < h; ++y, ofs += lineBytes) {
     uint8_t b[8];
     for (int i = 0; i < 8; ++i) b[i] = (uint8_t)(ofs >> (8 * i));
     f.write(reinterpret_cast<const char*>(b), 8);
   }
+  std::vector<float> row((size_t)w);
   for (int y = 0; y < h; ++y) {
     std::vector<uint8_t> l;
     put32(l, (uint32_t)y);
-    put32(l, (uint32_t)(w * 4));
+    put32(l, (uint32_t)(w * 4 * channels));
     f.write(reinterpret_cast<const char*>(l.data()), 8);
-    f.write(reinterpret_cast<const char*>(data + (size_t)y * w), (std::streamsize)w * 4);
+    for (int c = 0; c < channels; ++c) {
+      for (int x = 0; x < w; ++x) row[x] = data[((size_t)y * w + x) * channels + c];
+      f.write(reinterpret_cast<const char*>(row.data()), (std::streamsize)w * 4);
+    }
   }
   CHECK(f.good()) << "failed to save image: " << path.string();
 }
+inline void writeExrFloat(const fs::path& path, const float* data, int w, int h) { writeExrFloatChannels(path, data, w, h, 1); }
 
 // 16-bit PNG, `channels` = 1 (gray) or 3 (BGR input, written as RGB)
 inline void writePng16(const fs::path& path, const uint16_t* data, int w, int h, int channels) {
@@ -682,6 +692,35 @@ inline Image loadUnchanged(const fs::path& path) {
 }
 
 inline int cvRoundD(double v) { return (int)std::lrint(v); }
+
+// cv_util::loadImage<cv::Vec4f>: integer samples * (1 / max), alpha 1 when the file has none
+inline std::vector<float> loadColorF32x4(const fs::path& p, int* w, int* h) {
+  const Image img = loadUnchanged(p);
+  *w = img.w;
+  *h = img.h;
+  const size_t n = (size_t)img.w * img.h;
+  std::vector<float> out(n * 4);
+  const float scale = img.bits == 16 ? 1.0f / 65535.0f : 1.0f / 255.0f;
+  for (size_t i = 0; i < n; ++i)
+    for (int c = 0; c < 4; ++c) {
+      float v = 1.0f;
+      if (c < 3 || img.channels == 4) {
+        const size_t idx = i * img.channels + (img.channels >= 3 ? c : 0);
+        v = img.bits == 32 ? img.f[idx] : img.u[idx] * scale;
+      }
+      out[i * 4 + c] = v;
+    }
+  return out;
+}
+
+// image_util::verifyImagePaths: every camera has every frame of [first, last] (ext "" = the directory's first extension)
+inline void verifyImagePaths(const std::string& dir, const Rig& rig, int first, int last, const std::string& ext) {
+  for (const std::string& id : rig.ids)
+    for (int f = first; f <= last; ++f) {
+      const fs::path p = ext.empty() ? imagePath(dir, id, zeroPad(f)) : fs::path(dir) / id / (zeroPad(f) + ext);
+      CHECK(fs::exists(p)) << "missing file: " << p.string();
+    }
+}
 
 // loadImage<cv::Vec3w>: depth -> 16U (8U scaled by 65535/255 = 257, float by 65535 with rounding and
 // saturation), then channels -> 3 (gray replicated, alpha dropped)
