@@ -576,7 +576,7 @@ __global__ void rephotoPrepKernel(DevCamera cam, const float* disp, const float*
     texC[i] = make_ushort4(unorm16(c[0]), unorm16(c[1]), unorm16(c[2]), a);
   }
   if (texD) {
-    const double dist2 = 1.0 / (double)d;
+    const double dist2 = (float)(1.0 / (double)d);  // DisparityColor.h: float distance = 1.0 / disparity
     const float wx = (float)(cam.pos[0] + dir[0] * dist2), wy = (float)(cam.pos[1] + dir[1] * dist2),
                 wz = (float)(cam.pos[2] + dir[2] * dist2);
     const float ex = wx - cx, ey = wy - cy, ez = wz - cz;

@@ -50,6 +50,25 @@ def _views(lib, rig, disps, bgra, i):
     return ref, ren
 
 
+STEP = 1 / 65535 + 1e-6  # one RGBA16 step
+
+
+def check_disparity_colour(g, o, what):
+    """Disparity colour, GPU against checker.  Its texel 1 / |world - centre| starts from the fp64 camera ray, whose
+    sin / cos / atan may differ by an ulp between libdevice and glibc.  Both sides round the distance to fp32 first
+    (DisparityColor.h: float distance = 1.0 / disparity), which absorbs such an ulp except at an fp32 rounding
+    boundary, so a texel lands one RGBA16 step apart only rarely.  The blend is a convex combination of texels, so a
+    value can differ by at most that step.  Requires NaN at the same places, at most a few differing values in 10^6 and
+    none by more than one step."""
+    nan = np.isnan(o)
+    assert np.array_equal(np.isnan(g), nan), what
+    diff = np.abs(g - o)[~nan]
+    count, err = int((diff > 0).sum()), float(diff.max()) if diff.size else 0.0
+    print(what, "disparity colour: %d of %d values differ, max |cuda - oracle| %.3g" % (count, diff.size, err))
+    assert count <= 3e-6 * diff.size, (what, count, diff.size)
+    assert err <= STEP, (what, err)
+
+
 def _score(lib, ref, ren, method="MSSIM", radius=1):
     mask = (ref[0][..., 3] > 0).astype(np.uint8)
     return lib.rephoto_score(ref[0][..., :3], ren[0][..., :3], mask, method, radius)
@@ -72,15 +91,13 @@ def test_cubemaps_and_scores_match_oracle(rcuda, roracle, case):
         # coverage and every canopy's surviving primitive: same rules, same fp32/fp64 arithmetic -> bit for bit
         assert np.array_equal(gw, ow) and np.array_equal(rw, qw), (case, i, int((gw != ow).sum()), int((rw != qw).sum()))
         assert (rw >= 0).any(axis=0).mean() > (0.5 if case.startswith("ring") else 0.1)
-        for g, o, tol in ((gc, oc, 0.0), (gd, od, 1 / 65535 + 1e-6), (rc, qc, 0.0), (rd, qd, 1 / 65535 + 1e-6)):
+        for g, o in ((gc, oc), (rc, qc)):
+            # colour: the same RGBA16 texels, weights and fp32 sums -> the same bits
             assert np.array_equal(g[..., 3] > 0, o[..., 3] > 0)
-            # Colour: the same RGBA16 texels, weights and fp32 sums -> the same bits.  Disparity colour: its texel
-            # 1 / |world - centre| comes from the fp64 camera ray, whose sin / cos / atan differ by an ulp between
-            # libdevice and glibc, so a texel can land one RGBA16 step (1 / 65535) apart; the blend is a convex
-            # combination of texels, so the cubemap differs by at most that step.
-            err = float(np.abs(g - o).max())
-            print(case, i, "max |cuda - oracle|:", err)
-            assert err <= tol, (case, i, err)
+            assert np.array_equal(g, o), (case, i, float(np.abs(g - o).max()))
+        for g, o in ((gd, od), (rd, qd)):
+            assert np.array_equal(g[..., 3] > 0, o[..., 3] > 0)
+            check_disparity_colour(g, o, (case, i))
         for method in ("MSSIM", "NCC"):
             for radius in (1, 2):
                 sg, ag = _score(rcuda, (gc,), (rc,), method, radius)

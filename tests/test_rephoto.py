@@ -1,6 +1,7 @@
 """ComputeRephotographyErrors without a GPU: the oracle's score against cv2 4.13 (tests/golden/rephoto_vectors.npz,
 generator tests/golden/gen_rephoto_vectors.py), properties of the oracle's cubemap render, and the app's command line."""
 import ctypes as C
+import hashlib
 import json
 import os
 import re
@@ -13,6 +14,9 @@ from facebook360_dep_b200 import capi, synth
 from tests import rephoto_oracle
 
 G = np.load(os.path.join(os.path.dirname(__file__), "golden", "rephoto_vectors.npz"))
+# the same score at edge shapes and radii (generator tests/golden/gen_rephoto_edge_vectors.py)
+E = np.load(os.path.join(os.path.dirname(__file__), "golden", "rephoto_edge_vectors.npz"))
+EDGE_CASES = ("odd", "cube", "tiny", "row", "col", "empty")
 HOST = os.path.join(capi.ROOT, "facebook360_dep_b200", "csrc", "host")
 APP = os.path.join(capi.ROOT, "facebook360_dep_b200", "bin", "ComputeRephotographyErrors")
 
@@ -23,18 +27,59 @@ def oracle():
     return rephoto_oracle.load()
 
 
+def check_score_vs_cv2(score, avg, ref, ref_avg, mask):
+    """test_score_matches_cv2's comparison: NaN where cv2 has NaN, scores within 1e-5, averages within 1e-6.  The
+    tolerance is the class of cv2's float filters (test_oracle_cv.py): SIMD / FMA-dispatched sums, 1e-6 of the value
+    scale per blur, amplified by the SSIM quotients."""
+    nan = np.isnan(ref)
+    assert np.array_equal(np.isnan(score), nan), int((np.isnan(score) != nan).sum())
+    if not nan.all():
+        assert np.abs(score - ref)[~nan].max() <= 1e-5, np.abs(score - ref)[~nan].max()
+    assert np.abs(avg - ref_avg).max() <= 1e-6, (avg, ref_avg)
+    if not mask.any():
+        assert np.array_equal(avg, np.zeros(3))  # cv::mean over an empty mask
+
+
+def edge_case(case, method, radius):
+    """(x, y, mask, cv2 score, cv2 averages) of one edge-shape vector set"""
+    return (E[case + "_x"], E[case + "_y"], E[case + "_mask"], E["%s_score_%s_r%d" % (case, method, radius)],
+            E["%s_avg_%s_r%d" % (case, method, radius)])
+
+
 @pytest.mark.parametrize("method", ["MSSIM", "NCC"])
-@pytest.mark.parametrize("radius", [1, 2])
+@pytest.mark.parametrize("radius", [1, 2, 4, 5, 31])
 def test_score_matches_cv2(oracle, method, radius):
     score, avg = oracle.rephoto_score(G["x"], G["y"], G["mask"], method, radius)
-    ref = G["score_%s_r%d" % (method, radius)]
+    src = G if radius <= 2 else {k[5:]: E[k] for k in E.files if k.startswith("base_")}
+    ref = src["score_%s_r%d" % (method, radius)]
     nan = np.isnan(ref)
     assert nan.any() and (nan[..., 0] & (G["mask"] > 0)).any()  # NaN scores inside the mask are part of the case
-    assert np.array_equal(np.isnan(score), nan)
-    # tolerance class of cv2's float filters (test_oracle_cv.py): SIMD / FMA-dispatched sums, 1e-6 of the value scale
-    # per blur, amplified by the SSIM quotients
-    assert np.abs(score - ref)[~nan].max() <= 1e-5, np.abs(score - ref)[~nan].max()
-    assert np.abs(avg - G["avg_%s_r%d" % (method, radius)]).max() <= 1e-6
+    assert (~nan[..., 0] & (G["mask"] > 0)).any()
+    check_score_vs_cv2(score, avg, ref, src["avg_%s_r%d" % (method, radius)], G["mask"])
+
+
+@pytest.mark.parametrize("method", ["MSSIM", "NCC"])
+@pytest.mark.parametrize("radius", [1, 2, 4, 5, 31])
+@pytest.mark.parametrize("case", EDGE_CASES)
+def test_score_edge_shapes_match_cv2(oracle, case, method, radius):
+    """Odd non-square and cubemap-layout images, kernels wider than the image (reflect101 bouncing several times),
+    1-pixel-wide and -tall images, NaN inputs inside the mask and an empty mask."""
+    x, y, mask, ref, ref_avg = edge_case(case, method, radius)
+    score, avg = oracle.rephoto_score(x, y, mask, method, radius)
+    check_score_vs_cv2(score, avg, ref, ref_avg, mask)
+
+
+def test_golden_score_vectors_unchanged():
+    """rephoto_vectors.npz is the cv2 pin the GPU and CPU tests share; the edge vectors live in a file of their own."""
+    h = hashlib.sha256()
+    for k in sorted(G.files):
+        a = G[k]
+        h.update(k.encode())
+        h.update(str(a.dtype).encode())
+        h.update(str(a.shape).encode())
+        h.update(np.ascontiguousarray(a).tobytes())
+    assert len(G.files) == 18 and h.hexdigest() == "a6bd991d35e2b4bc67ebb7bf030c35581f06e04141ee3d065ba5282e234a9583"
+    assert not any(k.startswith("base_") and k[5:] in G.files for k in E.files)
 
 
 def _jet(oracle, score, mask):
