@@ -24,13 +24,6 @@
 #include <cstdint>
 #include <cstring>
 
-#ifndef DERP_BC7_MIN_CTAS  // build-time experiment knobs
-#define DERP_BC7_MIN_CTAS 2
-#endif
-#ifndef DERP_BC7_RANK_UNROLL
-#define DERP_BC7_RANK_UNROLL 1
-#endif
-
 namespace derp {
 namespace bc7 {
 
@@ -128,6 +121,7 @@ struct HostPixels {
 };
 #ifdef __CUDACC__
 constexpr int kBc7Threads = 128;
+constexpr int kBc7MinCtas = 2;  // resident CTAs per SM bc7Kernel is compiled for (register cap)
 __shared__ float bc7Tile[48 * kBc7Threads];  // 24 KB per CTA; a thread only ever touches its own 48 words: no barriers
 struct SharedPixels {
   __device__ __forceinline__ float operator()(int c, int k) const { return bc7Tile[(c * 16 + k) * kBc7Threads + threadIdx.x]; }
@@ -578,8 +572,7 @@ BC7_FN void encodeBlock(const Px& px, uint32_t (&out)[4]) {
   {
     const Moments all = momentsOf(px, 0xFFFFu);
     int key0 = INT_MAX, key1 = INT_MAX, key2 = INT_MAX;
-    constexpr int kRankUnroll = DERP_BC7_RANK_UNROLL;
-#pragma unroll kRankUnroll
+#pragma unroll 1
     for (int part = 0; part < 64; ++part) {
       const Moments first = momentsOf(px, ~subset1Mask(part) & 0xFFFFu);
       float bound = 0;
@@ -684,7 +677,7 @@ struct BgrSource {
   }
 };
 template <typename Source>
-__global__ void __launch_bounds__(kBc7Threads, DERP_BC7_MIN_CTAS) bc7Kernel(Source src, int width, int blocksX, int blocksY, uint8_t* out) {
+__global__ void __launch_bounds__(kBc7Threads, kBc7MinCtas) bc7Kernel(Source src, int width, int blocksX, int blocksY, uint8_t* out) {
   const int b = blockIdx.x * kBc7Threads + threadIdx.x;
   if (b >= blocksX * blocksY) return;
   const int bx = b % blocksX, by = b / blocksX;

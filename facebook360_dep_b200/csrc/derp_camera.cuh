@@ -31,15 +31,10 @@ struct alignas(16) DevCamera {
   int type;
   int defaultFov;       // cosFov == getDefaultCosFov(type) (Camera.cpp:206-208)
   int zeroDist;         // getDistortion().isZero() (Camera.h:256)
-  int coneMode;         // 0: general cone test, 1: cosFov == -1 (never outside), 2: cosFov == 0 (isBehind)
-  // fp32 copies for the conservative pre-test of isOutsideFov (derp_cost.cuh::coneClass): position, forward axis
-  // (= -rot row 2), cosFov * |cosFov| and the 1-norm of the position
-  float conePos[3];
-  float coneC2;
-  float coneFwd[3];
-  float conePosL1;
+  int reserved[9];      // unused, zero
 };
 static_assert(sizeof(DevCamera) % 16 == 0, "DevCamera is staged with 128-bit copies");
+static_assert(sizeof(DevCamera) == 240, "the size sets the cost kernels' shared memory and so the sweep's CTA height");
 
 // ------------------------------------------------------------------------------------------------
 // Host-side construction
@@ -223,13 +218,6 @@ inline bool makeCamera(const DerpCameraDesc& d, DevCamera* out) {
     c.cosFov = defaultCosFov(d.type);
   }
   c.defaultFov = (c.cosFov == defaultCosFov(d.type));
-  c.coneMode = c.cosFov == -1 ? 1 : (c.cosFov == 0 ? 2 : 0);
-  for (int i = 0; i < 3; ++i) {
-    c.conePos[i] = (float)c.pos[i];
-    c.coneFwd[i] = (float)(-c.rot[6 + i]);
-  }
-  c.coneC2 = (float)(c.cosFov * std::fabs(c.cosFov));
-  c.conePosL1 = (float)(std::fabs(c.pos[0]) + std::fabs(c.pos[1]) + std::fabs(c.pos[2]));
   *out = c;
   return true;
 }

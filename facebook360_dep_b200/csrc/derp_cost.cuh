@@ -18,12 +18,6 @@
 #include <cfloat>
 #include <cstdint>
 
-// Table-driven robust-mean selection (derp_select.cuh::robustSumTable), bit-exact with the general introselect
-// emulation on all parity tests; -DDERP_NO_SELECT_TABLE builds the general emulation only (the A/B baseline).
-#if !defined(DERP_NO_SELECT_TABLE) && !defined(DERP_SELECT_TABLE)
-#define DERP_SELECT_TABLE 1
-#endif
-
 #include "derp_camera.cuh"
 #include "derp_select.cuh"
 
@@ -46,9 +40,7 @@ struct CostView {
   // half-size texels halve the cache lines a request touches; the conversion costs 4 instructions per texel.
   const uint2* projColor16;
   const uint2* projBias16;
-#ifdef DERP_SELECT_TABLE
   const unsigned* selTab;  // robustSumTable's permutation table (derp_select.cuh)
-#endif
   const float2* projWarp;   // [S][H][W]  src px -> dst px at infinity (self slot unused)
   const float* variance;    // destination's own variance [H][W]
   const DevCamera* cams;    // [S] normalised cameras (global memory; staged to smem by kernels)
@@ -91,17 +83,7 @@ __device__ __forceinline__ Texel texelOf(float4 t) { return Texel{t.x, t.y, t.z}
 __device__ __forceinline__ float4 ldTexel(const float4* p) { return __ldg(p); }
 __device__ __forceinline__ float4 ldTexel(const uint2* p) {
   const uint2 t = __ldg(p);
-#ifdef DERP_U16_PRMT
-  // u16 -> f32 without the conversion unit: one byte permute builds the float 2^23 + u (0x4B00'uuuu), one add removes
-  // the 2^23 — two full-rate instructions instead of a quarter-rate I2F; exact for every u < 2^16
-  const float b = 8388608.0f;
-  return make_float4(__uint_as_float(__byte_perm(t.x, 0x4B000000u, 0x7610)) - b,
-                     __uint_as_float(__byte_perm(t.x, 0x4B000000u, 0x7632)) - b,
-                     __uint_as_float(__byte_perm(t.y, 0x4B000000u, 0x7610)) - b,
-                     __uint_as_float(__byte_perm(t.y, 0x4B000000u, 0x7632)) - b);
-#else
   return make_float4((float)(t.x & 0xffffu), (float)(t.x >> 16), (float)(t.y & 0xffffu), (float)(t.y >> 16));
-#endif
 }
 template <class TX>
 struct TablesOf;
@@ -202,10 +184,8 @@ __device__ __forceinline__ f32x2 bilerp2(f32x2 p00, f32x2 p01, f32x2 p10, f32x2 
 // Two float2 planes so that the two-lane arithmetic gets its operands with 64-bit shared loads:
 //   bg[row][col] = (B, G),   rr[row][col] = (R(row), R(row+1))   (vertical pair: see the R channel below)
 constexpr int kTileW = 32 + 2;
-#ifndef DERP_SWEEP_MAXBY
-#define DERP_SWEEP_MAXBY 20  // tallest CTA the sweep is launched with (32 x 20 threads => 96 registers, 20 warps/SM)
-#endif
-constexpr int kMaxTileH = DERP_SWEEP_MAXBY + 2;
+constexpr int kSweepMaxRows = 20;  // tallest CTA the sweep is launched with (32 x 20 threads => 96 registers, 20 warps/SM)
+constexpr int kMaxTileH = kSweepMaxRows + 2;
 constexpr int kTileFloats = 2 * kMaxTileH * kTileW * 2;
 
 // `addend`: 2^23 for the exact cost (see truncBiased), 0.5 for the lower-bound pass (midpoint of the truncation interval).
@@ -270,26 +250,16 @@ __device__ __forceinline__ void loadPixelState(const CostView& v, const DevCamer
 
 // Compacted kernels (one thread per ACTIVE pixel, pixels of a CTA are not a rectangle): every thread keeps its
 // own 3x3 patch in shared memory, laid out [row][col][thread] so that a warp reads consecutive words.
-#ifndef DERP_PATCH_THREADS
-#define DERP_PATCH_THREADS 256
-#endif
-#ifndef DERP_PATCH_MINB
+constexpr int kPatchThreads = 256;
 // Resident CTAs per SM the compacted kernels are compiled for (register cap).  2 => 128 registers, 16 warps/SM: these
 // kernels are L1-bound (scattered 4x4 gathers), so spill traffic costs more than the lost warps.
-#define DERP_PATCH_MINB 2
-#endif
-constexpr int kPatchThreads = DERP_PATCH_THREADS;
+constexpr int kPatchMinCtas = 2;
 constexpr int kPatchRP = 3 * kPatchThreads, kPatchCP = kPatchThreads;
 constexpr int kPatchFloats = 2 * 9 * kPatchThreads * 2;
 // pingPongKernel has its own CTA shape: 128 threads x 5 CTAs per SM (96 registers, 20 warps/SM), while proposalKernel
 // keeps 256 x 2 (it spills more at 96 registers).
-#ifndef DERP_PING_THREADS
-#define DERP_PING_THREADS 128
-#endif
-#ifndef DERP_PING_MINB
-#define DERP_PING_MINB 5
-#endif
-constexpr int kPingThreads = DERP_PING_THREADS;
+constexpr int kPingThreads = 128;
+constexpr int kPingMinCtas = 5;
 
 template <int T>
 __device__ __forceinline__ void loadPixelStateCompact(const CostView& v, const DevCamera& camDst, float* patches, int x,
@@ -368,51 +338,6 @@ __device__ __forceinline__ bool insideCone(const DevCamera& c, double wx, double
   return !(dot * fabs(dot) <= c.cosFov * fabs(c.cosFov) * n2);
 }
 
-// The fields of the cone test alone, for kernels that pass them BY VALUE in their parameter block: the candidate loop
-// of the dense sweep tests every source for every candidate with a warp-uniform source index, so reading the seven doubles
-// from the constant bank (uniform loads / constant operands) instead of shared memory takes that traffic off the
-// L1 / shared-memory pipe the sweep is limited by.
-struct ConeCam {
-  double pos[3];
-  double back[3];  // rotation row 2 (= -forward)
-  double cosFov;
-  double pad;
-};
-__device__ __forceinline__ bool insideCone(const ConeCam& c, double wx, double wy, double wz) {
-  if (c.cosFov == -1) return true;
-  const double vx = wx - c.pos[0], vy = wy - c.pos[1], vz = wz - c.pos[2];
-  const double camz = c.back[0] * vx + c.back[1] * vy + c.back[2] * vz;
-  if (c.cosFov == 0) return !(camz >= 0);  // !isBehind
-  const double dot = -camz;
-  const double n2 = vx * vx + vy * vy + vz * vz;
-  return !(dot * fabs(dot) <= c.cosFov * fabs(c.cosFov) * n2);
-}
-
-// Conservative fp32 version of the same test (-DDERP_CONE_F32; built and validated, off by default: the fp64 pipe is not
-// the binding resource of the sweep):
-// 1 = inside, 0 = outside, -1 = too close to call (the caller then runs insideCone in fp64, so the decision is ALWAYS the
-// reference's).
-// Error bound (u = 2^-24, |.|_1 the 1-norm, B = |w|_1 + |pos|_1 >= |v|_1 >= |v|_2): every component of
-// v = fl(fl(w) - fl(pos)) is off by at most u(|w_i| + |pos_i| + |v_i|) <= 2uB; the forward axis is a unit vector
-// rounded to fp32, so dot = f.v (three rounded operations) is off by at most |f|_2 |dv|_2 + 4u|v| < 8uB; n2 = v.v by at most
-// 4|v|uB*sqrt(3) + 3u n2 < 10uB^2; hence lhs - rhs = dot|dot| - c2 n2 (|c2| <= 1, c2 rounded: +u) is off by less than
-// 2B*8uB + (8uB)^2 + 10uB^2 + 3uB^2 < 30uB^2.  The margin used is 64uB^2 = 2^-18 B^2 (2^-20 B on dot for the hemisphere
-// case, bound 8uB = 2^-21 B).  NaN / infinite inputs fail both comparisons and fall through to the fp64 test.
-__device__ __forceinline__ int coneClass(const DevCamera& c, float wx, float wy, float wz, float wL1) {
-  if (c.coneMode == 1) return 1;
-  const float vx = wx - c.conePos[0], vy = wy - c.conePos[1], vz = wz - c.conePos[2];
-  const float dot = __fmaf_rn(c.coneFwd[2], vz, __fmaf_rn(c.coneFwd[1], vy, c.coneFwd[0] * vx));
-  const float B = wL1 + c.conePosL1;
-  if (c.coneMode == 2) {  // inside iff !(camz >= 0) iff forward . v > 0
-    const float m = 9.5367431640625e-07f * B;  // 2^-20 B
-    return dot > m ? 1 : (dot < -m ? 0 : -1);
-  }
-  const float n2 = __fmaf_rn(vz, vz, __fmaf_rn(vy, vy, vx * vx));
-  const float d = __fmaf_rn(-c.coneC2, n2, dot * fabsf(dot));  // inside iff !(dot|dot| <= c2 n2) iff d > 0
-  const float m = 3.814697265625e-06f * (B * B);  // 2^-18 B^2
-  return d > m ? 1 : (d < -m ? 0 : -1);
-}
-
 // pixel() + isOutsideSensor + de-normalisation + narrowing (Camera.h:121-128,180-190, DerpUtil.cpp:56-73,
 // Derp.cpp:175) for a point that already passed the cone test.  Straight-line code (no early exit) so that
 // the scheduler can interleave it with the fp32 SSD of the previous source.
@@ -437,34 +362,6 @@ __device__ __forceinline__ SrcPoint projectToSource(const DevCamera& c, double w
   o.y = (float)py;
   return o;
 }
-
-#ifdef DERP_EXPERIMENT_PROJ_F32
-// TIMING EXPERIMENT ONLY (results of the lower-bound pass are not valid bounds in this build): the projection of the
-// lower-bound pass in fp32, to measure what an fp32 projection with a position-error analysis could save at most.
-__device__ __forceinline__ SrcPoint projectToSourceF32(const DevCamera& c, float wx, float wy, float wz, int W, int H) {
-  const float vx = wx - c.conePos[0], vy = wy - c.conePos[1], vz = wz - c.conePos[2];
-  const float r0 = (float)c.rot[0], r1 = (float)c.rot[1], r2 = (float)c.rot[2], r3 = (float)c.rot[3], r4 = (float)c.rot[4],
-              r5 = (float)c.rot[5];
-  const float camx = __fmaf_rn(r2, vz, __fmaf_rn(r1, vy, r0 * vx));
-  const float camy = __fmaf_rn(r5, vz, __fmaf_rn(r4, vy, r3 * vx));
-  const float camz = -__fmaf_rn(c.coneFwd[2], vz, __fmaf_rn(c.coneFwd[1], vy, c.coneFwd[0] * vx));
-  const float xy2 = __fmaf_rn(camy, camy, camx * camx);
-  const float inv = rsqrtf(xy2), xy = xy2 * inv;
-  float r = atan2f(xy, -camz);
-  const float dm = (float)c.distMax;
-  r = r < dm ? r : dm;
-  const float q = r * r;
-  const float fac = __fmaf_rn(q, __fmaf_rn(q, __fmaf_rn(q, (float)c.dist[2], (float)c.dist[1]), (float)c.dist[0]), 1.0f);
-  const float f = fac * r * inv;
-  const float px = __fmaf_rn((float)c.focal[0], f * camx, (float)c.principal[0]);
-  const float py = __fmaf_rn((float)c.focal[1], f * camy, (float)c.principal[1]);
-  SrcPoint o;
-  o.ok = !(0 > px || px >= 1.0f || 0 > py || py >= 1.0f);
-  o.x = px * W;
-  o.y = py * H;
-  return o;
-}
-#endif
 
 // Generic (border / inconsistent-rounding / invalid) path of one source: returns false if the source
 // contributes no SSD (warp entry NaN).  Kept out of line: it runs for a few pixels per image.
@@ -663,8 +560,7 @@ __device__ __forceinline__ int lowestSetBit(uint64_t m) { return __ffsll(m) - 1;
 // error bound, and the return value is a number that is <= the exact cost (0 = "unknown", FLT_MAX = no source).
 template <class Mask, int RP, int CP, class TX = float4, bool LOWER = false>
 __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __restrict__ cams,
-                                          const PixelState& ps, float disparity, unsigned* hits,
-                                          const ConeCam* __restrict__ cone = nullptr) {
+                                          const PixelState& ps, float disparity, unsigned* hits) {
   const double depth = (double)(1.0f / disparity);
   const DevCamera& cd = cams[v.self];
   const double wx = cd.pos[0] + ps.dir[0] * depth;
@@ -676,26 +572,9 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
   const f32x2 one2 = pk(one, one), b232 = pk(b23, b23), half2 = pk(0.5f, 0.5f);
 
   Mask mask = 0;
-  {
-    const float fx = (float)wx, fy = (float)wy, fz = (float)wz;
-    const float wL1 = fabsf(fx) + fabsf(fy) + fabsf(fz);
 #pragma unroll 4
-    for (int s = 0; s < v.S; ++s) {
-#if defined(DERP_EXPERIMENT_PROJ_F32)
-      int cls = -1;
-      if constexpr (LOWER) {
-        cls = coneClass(cams[s], fx, fy, fz, wL1);
-        cls = cls < 0 ? 1 : cls;
-      }
-#elif defined(DERP_CONE_F32)
-      const int cls = coneClass(cams[s], fx, fy, fz, wL1);
-#else
-      const int cls = -1;
-#endif
-      const bool in = cls < 0 ? (cone ? insideCone(cone[s], wx, wy, wz) : insideCone(cams[s], wx, wy, wz)) : (cls != 0);
-      if (in) mask |= Mask(1) << s;
-    }
-  }
+  for (int s = 0; s < v.S; ++s)
+    if (insideCone(cams[s], wx, wy, wz)) mask |= Mask(1) << s;
   mask &= ~(Mask(1) << v.self);
 
   // (biased, unbiased) SSD of every contributing source: this thread's column of the [slot][thread] array in shared
@@ -730,15 +609,10 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
     t.yw = hi2(Wt);
     return t;
   };
-#ifdef DERP_EXPERIMENT_PROJ_F32
-#define DERP_PROJECT(cam) (LOWER ? projectToSourceF32(cam, (float)wx, (float)wy, (float)wz, W, H) : projectToSource(cam, wx, wy, wz, W, H))
-#else
-#define DERP_PROJECT(cam) projectToSource(cam, wx, wy, wz, W, H)
-#endif
   if (mask) {
     int s = lowestSetBit(mask);
     mask &= mask - 1;
-    SrcPoint cur = DERP_PROJECT(cams[s]);
+    SrcPoint cur = projectToSource(cams[s], wx, wy, wz, W, H);
     while (true) {
       // Tail (!more): the exact path re-projects the same source, harmlessly, to keep its main block straight-line
       // code.  The lower-bound pass skips that projection: in a warp's last iteration no lane needs it, and measured
@@ -785,7 +659,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
           const TX* r3 = r2 + W;
           const TX* b1 = srcBiasImg + off + W + 1;  // bias sample = centre sample's 2x2 footprint
           if constexpr (LOWER) {
-            if (more) nxt = DERP_PROJECT(cams[sNext]);
+            if (more) nxt = projectToSource(cams[sNext], wx, wy, wz, W, H);
             float sB, sU;
             ssdApprox<RP, CP>(r0, r1, r2, r3, b1, W, ps, W0, W1, W2, &sB, &sU);
             // slot = (sqrt of the biased sum, lower bound of the unbiased sum), see lowerBoundOfCost
@@ -793,12 +667,7 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
             const float ul = fmaxf(rU - kErrU, 0.0f);
             pushPair(rB, ul * ul);
           } else {
-#ifdef DERP_EXPERIMENT_NOBIAS  // measurement-only variant (breaks parity): upper bound of not reading the bias table
-          const float4 q00 = make_float4(1.f, 2.f, 3.f, 0.f), q01 = q00, q10 = q00, q11 = q00;
-          (void)b1;
-#else
           const float4 q00 = ldTexel(b1), q01 = ldTexel(b1 + 1), q10 = ldTexel(b1 + W), q11 = ldTexel(b1 + W + 1);
-#endif
           float4 colA[4], colB[4];
           colA[0] = ldTexel(r0);
           colA[1] = ldTexel(r1);
@@ -910,15 +779,14 @@ __device__ __forceinline__ float evalCost(const CostView& v, const DevCamera* __
     }
     cost = 0.0f + m.y;
   } else if (n <= kSelSlots) {
-#ifdef DERP_SELECT_TABLE  // host-validated on every permutation (tests/test_host_units.py), GPU-validated by the parity suite
+    // table-driven selection: host-validated on every permutation (tests/test_host_units.py), GPU-validated by the
+    // parity suite; it declines ties and NaNs, which take the general algorithm
     static_assert(kSelSlots <= kSelTabMaxN, "the table path covers every evaluation that fits the shared-memory slots");
     // the 15-compare instance when no lane of the warp that got here holds more than 6 pairs
     const bool small = __reduce_max_sync(__activemask(), (unsigned)n) <= 6u;
     const bool done = small ? robustSumTable<6>(SmemPairs{ps.sel, ps.selStride}, n, keep, v.selTab, &cost)
                             : robustSumTable<8>(SmemPairs{ps.sel, ps.selStride}, n, keep, v.selTab, &cost);
-    if (!done)
-#endif
-      cost = robustSum(SmemPairs{ps.sel, ps.selStride}, n, keep);
+    if (!done) cost = robustSum(SmemPairs{ps.sel, ps.selStride}, n, keep);
   } else {  // more than kSelTabMaxN sources: the general algorithm on the shared-memory slots
     cost = robustSum(SmemPairs{ps.sel, ps.selStride}, n, keep);
   }

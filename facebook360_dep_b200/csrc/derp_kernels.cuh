@@ -14,9 +14,7 @@ namespace derp {
 
 constexpr int kBlockX = 32, kBlockY = 8;  // 256 threads
 // resident CTAs per SM requested for the cost kernels: 3 -> 80 registers, 24 warps/SM
-#ifndef DERP_SWEEP_MINB
-#define DERP_SWEEP_MINB 3
-#endif
+constexpr int kCostMinCtas = 3;
 
 __device__ __forceinline__ void stageCameras(DevCamera* sm, const DevCamera* __restrict__ g, int n) {
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
@@ -353,15 +351,13 @@ struct SweepArgs {
   unsigned long long* counters;  // [0] cost evaluations, [1] source hits
 };
 
-// Launched with 32 x BY threads: BY = DERP_SWEEP_MAXBY (20 => one 640-thread CTA per SM at 96 registers) on levels of
-// >= 1024 rows, 8 on smaller ones; a taller CTA shares more texel rows between its warps (per-warp footprint (BY+3)/BY
+// Launched with 32 x BY threads: BY = kSweepMaxRows (20 => one 640-thread CTA per SM at 96 registers) on levels of
+// >= 1024 rows, 10 on smaller ones; a taller CTA shares more texel rows between its warps (per-warp footprint (BY+3)/BY
 // rows instead of 11/8).  Rigs of more than 42 cameras get shorter CTAs, whose S - 1 selection slots per thread still fit
 // in shared memory (DerpCtx::sweepRows).
-#ifndef DERP_SWEEP_CTAS
-#define DERP_SWEEP_CTAS 1
-#endif
+constexpr int kSweepMinCtas = 1;
 template <class Mask>
-__global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepKernel(const SweepArgs a) {
+__global__ void __launch_bounds__(32 * kSweepMaxRows, kSweepMinCtas) sweepKernel(const SweepArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* tile = reinterpret_cast<float*>(cams + a.v.S);
@@ -384,11 +380,7 @@ __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepK
       for (int c = c0; c < c1; ++c) {
         const float d = __ldg(a.disparities + c);
         if (a.bg && !(bgd < d)) continue;  // closerMask (Derp.cpp:240-243)
-#ifdef DERP_SWEEP_U16  // measurement variant: the dense sweep on the 8-byte u16 tables
-        const float cost = evalCost<Mask, kTileW, 1, uint2>(a.v, cams, ps, d, &hits);
-#else
         const float cost = evalCost<Mask, kTileW, 1>(a.v, cams, ps, d, &hits);
-#endif
         ++evals;
         if (cost < bestCost) {
           bestCost = cost;
@@ -475,7 +467,7 @@ __global__ void extendBorderKernel(int W, int H, const uint8_t* __restrict__ fg,
 
 // ---- derp_eval_cost: one hypothesis per pixel ------------------------------------------------------
 template <class Mask>
-__global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB)
+__global__ void __launch_bounds__(kBlockX* kBlockY, kCostMinCtas)
     evalCostKernel(const CostView v, const float* __restrict__ disparity, float* __restrict__ outCost,
                    float* __restrict__ outConf, unsigned long long* counters) {
   extern __shared__ double smemRaw[];
@@ -617,7 +609,7 @@ __global__ void backgroundFillKernel(int W, int H, const uint8_t* __restrict__ f
 }
 
 template <class Mask>
-__global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) proposalKernel(const ProposalArgs a) {
+__global__ void __launch_bounds__(kPatchThreads, kPatchMinCtas) proposalKernel(const ProposalArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* patches = reinterpret_cast<float*>(cams + a.v.S);
@@ -698,7 +690,7 @@ __global__ void pingPongInitKernel(int W, int H, const uint8_t* __restrict__ fov
 }
 
 template <class Mask>
-__global__ void __launch_bounds__(kPingThreads, DERP_PING_MINB) pingPongKernel(const PingPongArgs a) {
+__global__ void __launch_bounds__(kPingThreads, kPingMinCtas) pingPongKernel(const PingPongArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* patches = reinterpret_cast<float*>(cams + a.v.S);

@@ -31,13 +31,10 @@ struct LowerArgs {
   float* lb;                   // [D][H][W]
   unsigned long long* seed;    // [H][W]  (L bits << 32 | candidate), atomicMin across candidate chunks
   unsigned long long* counters;
-#ifdef DERP_CONE_PARAMS
-  ConeCam cone[kNarrowMaxCams];  // cone-test fields of every camera, read from the constant bank (derp_cost.cuh)
-#endif
 };
 
 template <class Mask>
-__global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepLowerKernel(const LowerArgs a) {
+__global__ void __launch_bounds__(32 * kSweepMaxRows, kSweepMinCtas) sweepLowerKernel(const LowerArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* tile = reinterpret_cast<float*>(cams + a.v.S);
@@ -62,12 +59,7 @@ __global__ void __launch_bounds__(32 * DERP_SWEEP_MAXBY, DERP_SWEEP_CTAS) sweepL
         const float d = __ldg(a.disparities + c);
         float L = FLT_MAX;
         if (!(a.bg && !(bgd < d))) {  // closerMask (Derp.cpp:240-243)
-#ifdef DERP_CONE_PARAMS
-          // the parameter block holds kNarrowMaxCams cameras: wider rigs read the cone fields from shared memory
-          L = evalCost<Mask, kTileW, 1, float4, true>(a.v, cams, ps, d, &hits, sizeof(Mask) == 4 ? a.cone : nullptr);
-#else
           L = evalCost<Mask, kTileW, 1, float4, true>(a.v, cams, ps, d, &hits);
-#endif
           ++evals;
         }
         a.lb[c * plane + p] = L;
@@ -97,7 +89,7 @@ struct SeedArgs {
 
 // exact cost of the seed candidate; same CTA shape and shared-memory layout as evalCostKernel
 template <class Mask>
-__global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) sweepSeedKernel(const SeedArgs a) {
+__global__ void __launch_bounds__(kBlockX* kBlockY, kCostMinCtas) sweepSeedKernel(const SeedArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* tile = reinterpret_cast<float*>(cams + a.v.S);
@@ -171,7 +163,7 @@ struct RefineArgs {
 };
 
 template <class Mask>
-__global__ void __launch_bounds__(kPatchThreads, DERP_PATCH_MINB) refineKernel(const RefineArgs a) {
+__global__ void __launch_bounds__(kPatchThreads, kPatchMinCtas) refineKernel(const RefineArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* patches = reinterpret_cast<float*>(cams + a.v.S);
@@ -203,7 +195,7 @@ struct CheckArgs {
 };
 
 template <class Mask>
-__global__ void __launch_bounds__(kBlockX* kBlockY, DERP_SWEEP_MINB) lowerBoundCheckKernel(const CheckArgs a) {
+__global__ void __launch_bounds__(kBlockX* kBlockY, kCostMinCtas) lowerBoundCheckKernel(const CheckArgs a) {
   extern __shared__ double smemRaw[];
   DevCamera* cams = reinterpret_cast<DevCamera*>(smemRaw);
   float* tile = reinterpret_cast<float*>(cams + a.v.S);

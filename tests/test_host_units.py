@@ -190,9 +190,9 @@ def _table(prod, a, b, keep):
 
 
 def test_table_driven_selection_equals_general_algorithm(prod):
-    """derp_select.cuh's permutation-table path (a round-2 candidate for the cost kernels, compiled in with
-    -DDERP_SELECT_TABLE) against the general libstdc++-order algorithm that the kernels run today: every permutation
-    for n = 4..8, bit-identical fp32 sums; ties / NaNs in the first key must be declined."""
+    """derp_select.cuh's permutation-table path, which the cost kernels use for 4..8 sources, against the general
+    libstdc++-order algorithm they fall back to: every permutation for n = 4..8, bit-identical fp32 sums; ties / NaNs
+    in the first key must be declined."""
     import itertools
     rng = np.random.RandomState(11)
     checked = 0
