@@ -722,3 +722,132 @@ def load_cuda():
             raise RuntimeError("%s reports backend %r, expected the CUDA library" % (CUDA_LIB, lib.backend))
         _cache["cuda"] = lib
     return _cache["cuda"]
+
+
+# ---- include/derp_sweepview.h -------------------------------------------------------------------------------------
+_SWEEP_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_sweep_overlaps": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, _p(C.c_void_p), C.c_void_p, C.c_int, C.c_void_p,
+                                      C.c_int, C.c_void_p]),
+    "derp_sweep_crop_bounds": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_int,
+                                         C.c_void_p]),
+    "derp_sweep_equirect": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, C.c_int, _p(C.c_void_p), C.c_void_p, C.c_uint64,
+                                      C.c_void_p, C.c_int, C.c_void_p, C.c_int, _p(C.c_void_p)]),
+    "derp_sweep_center_rig": (C.c_int, [_p(CameraDesc), C.c_int, C.c_int, _p(CameraDesc), C.c_void_p]),
+    "derp_sweep_last_hits": (C.c_uint64, []),
+}
+SWEEP_SYMBOLS = sorted(k for k in _SWEEP_SIGS if k.startswith("derp_sweep_")) + ["derp_sweep_crop_width"]
+SWEEP_TEST_HOOKS = ["derp_test_sweep_equirect_host", "derp_test_sweep_overlaps_host"]
+
+
+def rescaled_descs(descs, scale):
+    """The rig as GenerateCameraOverlaps / GenerateEquirect hold it after Camera::rescale(resolution * scale)
+    (Camera.cpp:217-223): resolution * scale, principal and focal times newResolution / resolution, in fp64."""
+    out = (CameraDesc * len(descs))()
+    for i, d in enumerate(descs):
+        r = CameraDesc()
+        C.pointer(r)[0] = d
+        for k in range(2):
+            res = d.resolution[k]
+            nr = res * scale
+            p = d.principal[k] if d.has_principal else res / 2
+            r.principal[k] = p * (nr / res)
+            r.focal[k] = d.focal[k] * (nr / res)
+            r.resolution[k] = nr
+        r.has_principal = 1
+        out[i] = r
+    return out
+
+
+class SweepView:
+    """ctypes binding of include/derp_sweepview.h on a loaded library: ``SweepView(load_cuda())`` for the product, or a
+    path to a library exporting some of the same entry points (the CPU checkers the tests build).  ``host=True`` runs
+    the product's DERP_HD per-pixel code on the host (derp_test_sweep_*_host)."""
+
+    def __init__(self, library, host=False):
+        path = library.path if isinstance(library, Library) else library
+        if not os.path.exists(path):
+            raise FileNotFoundError(path)
+        self.path, self.lib, self.host = path, C.CDLL(path, mode=C.RTLD_LOCAL), host
+        for name, (res, args) in _SWEEP_SIGS.items():
+            fn = getattr(self.lib, name, None)
+            if fn is not None:
+                fn.restype = res
+                fn.argtypes = args
+        if host:
+            for name, sig in (("derp_test_sweep_overlaps_host", "derp_sweep_overlaps"),
+                              ("derp_test_sweep_equirect_host", "derp_sweep_equirect")):
+                fn = getattr(self.lib, name)
+                fn.restype = C.c_int
+                fn.argtypes = _SWEEP_SIGS[sig][1][1:]  # the same arguments without the device
+
+    def _check(self, rc):
+        if rc != 0:
+            raise DerpError(rc, self.lib.derp_last_error().decode())
+
+    @staticmethod
+    def _images(images):
+        ims = [np.ascontiguousarray(x, np.float32) for x in images]
+        assert all(x.ndim == 3 and x.shape[2] == 4 for x in ims)
+        sizes = np.array([[x.shape[1], x.shape[0]] for x in ims], np.int32).reshape(-1)
+        return ims, sizes
+
+    def overlaps(self, descs, images, dst, disparities, device=0):
+        """projectSrcsToDst of camera `dst` at each disparity: float [n, int(res.y), int(res.x), 4] (B, G, R, A)."""
+        ims, sizes = self._images(images)
+        disp = np.ascontiguousarray(disparities, np.float32)
+        W, H = int(descs[dst].resolution[0]), int(descs[dst].resolution[1])
+        out = np.empty((len(disp), H, W, 4), np.float32)
+        if self.host:
+            rc = self.lib.derp_test_sweep_overlaps_host(descs, len(descs), _ptr_array(ims), sizes.ctypes.data, dst,
+                                                        disp.ctypes.data, len(disp), out.ctypes.data)
+        else:
+            rc = self.lib.derp_sweep_overlaps(device, descs, len(descs), _ptr_array(ims), sizes.ctypes.data, dst,
+                                              disp.ctypes.data, len(disp), out.ctypes.data)
+        self._check(rc)
+        return out
+
+    def crop_bounds(self, descs, height, depths, center=-1, device=0):
+        """createCroppedEquirect's box per depth: float64 [n, 4] = minX, maxX, minY, maxY."""
+        dep = np.ascontiguousarray(depths, np.float32)
+        out = np.empty((len(dep), 4), np.float64)
+        self._check(self.lib.derp_sweep_crop_bounds(device, descs, len(descs), center, height, dep.ctypes.data, len(dep),
+                                                    out.ctypes.data))
+        return out
+
+    def crop_width(self, height, box):
+        f = self.lib.derp_sweep_crop_width
+        f.restype = C.c_int
+        f.argtypes = [C.c_uint64, C.c_void_p, _p(C.c_uint64)]
+        b = np.ascontiguousarray(box, np.float64)
+        w = C.c_uint64()
+        self._check(f(height, b.ctypes.data, C.byref(w)))
+        return w.value
+
+    def equirect(self, descs, images, height, depths, bounds=None, black_bg=False, center=-1, widths=None, device=0):
+        """createEquirect (bounds None) or createCroppedEquirect per depth: a list of float [height, width_k, 4]."""
+        ims, sizes = self._images(images)
+        dep = np.ascontiguousarray(depths, np.float32)
+        b = None if bounds is None else np.ascontiguousarray(bounds, np.float64)
+        if widths is None:
+            widths = [2 * height] * len(dep) if b is None else [self.crop_width(height, b[k]) for k in range(len(dep))]
+        outs = [np.empty((height, w, 4), np.float32) for w in widths]
+        args = (descs, len(descs), center, _ptr_array(ims), sizes.ctypes.data, height, dep.ctypes.data, len(dep), _dp(b),
+                int(bool(black_bg)), _ptr_array(outs))
+        if self.host:
+            self._check(self.lib.derp_test_sweep_equirect_host(*args))
+        else:
+            self._check(self.lib.derp_sweep_equirect(device, *args))
+        return outs
+
+    def last_hits(self):
+        """(sample, camera) pairs whose camera saw the point in this thread's last overlaps / equirect call."""
+        return int(self.lib.derp_sweep_last_hits())
+
+    def center_rig(self, descs, center):
+        """centerRig: (centred descriptors, float64 [n, 3, 3] rotations, float64 [n, 3] origins)."""
+        out = (CameraDesc * len(descs))()
+        rot = np.empty((len(descs), 3, 3), np.float64)
+        self._check(self.lib.derp_sweep_center_rig(descs, len(descs), center, out, rot.ctypes.data))
+        org = np.array([[out[i].origin[k] for k in range(3)] for i in range(len(descs))], np.float64)
+        return out, rot, org

@@ -75,6 +75,10 @@ inline std::string toStr(const bool& v) { return v ? "true" : "false"; }
 #define DEFINE_int32(name, def, help)                                                                   \
   DERP_DEFINE_FLAG(int, "int32", name, def, help, char* e = nullptr; long x = std::strtol(v.c_str(), &e, 10); \
                    if (v.empty() || *e) return false; FLAGS_##name = (int)x; return true;)
+#define DEFINE_uint64(name, def, help)                                                                  \
+  DERP_DEFINE_FLAG(uint64_t, "uint64", name, def, help, char* e = nullptr;                                   \
+                   unsigned long long x = std::strtoull(v.c_str(), &e, 10);                                   \
+                   if (v.empty() || *e || v[0] == '-') return false; FLAGS_##name = (uint64_t)x; return true;)
 #define DEFINE_double(name, def, help)                                                                  \
   DERP_DEFINE_FLAG(double, "double", name, def, help, char* e = nullptr; double x = std::strtod(v.c_str(), &e); \
                    if (v.empty() || *e) return false; FLAGS_##name = x; return true;)
