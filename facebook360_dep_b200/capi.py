@@ -182,24 +182,38 @@ class DerpError(RuntimeError):
         self.code = code
 
 
-class Library:
+def _bind(library, sigs, optional=()):
+    """Opens `library` (a path, or a binding of one) and sets restype and argtypes of every entry point in `sigs`.
+    Returns (path, CDLL).  A missing entry point raises AttributeError unless its name is in `optional`."""
+    path = getattr(library, "path", library)
+    if not os.path.exists(path):
+        raise FileNotFoundError(
+            "%s not found — build it first (python -c 'import __graft_entry__ as g; g.build()')" % path)
+    lib = C.CDLL(path, mode=C.RTLD_LOCAL)
+    for name, (res, args) in sigs.items():
+        fn = getattr(lib, name, None) if name in optional else getattr(lib, name)
+        if fn is not None:
+            fn.restype = res
+            fn.argtypes = args
+    return path, lib
+
+
+class _Binding:
+    """A library whose entry points return a DERP_* code and leave the message in derp_last_error."""
+
+    def _check(self, rc):
+        if rc != 0:
+            raise DerpError(rc, self.lib.derp_last_error().decode())
+
+
+class Library(_Binding):
     """One loaded shared library exporting the derp_b200.h ABI."""
 
     def __init__(self, path):
-        if not os.path.exists(path):
-            raise FileNotFoundError(
-                "%s not found — build it first (python -c 'import __graft_entry__ as g; g.build()')" % path)
-        self.path = path
-        self.lib = C.CDLL(path, mode=C.RTLD_LOCAL)
-        for name, (res, args) in _SIGS.items():
-            fn = getattr(self.lib, name)  # AttributeError if a declared symbol is missing
-            fn.restype = res
-            fn.argtypes = args
+        self.path, self.lib = _bind(path, _SIGS)
         self.backend = self.lib.derp_backend().decode()
 
-    def check(self, rc):
-        if rc != 0:
-            raise DerpError(rc, self.lib.derp_last_error().decode())
+    check = _Binding._check
 
     def set_threads(self, n):
         self.check(self.lib.derp_set_threads(int(n)))
@@ -326,25 +340,12 @@ REPHOTO_SYMBOLS = sorted(k for k in _REPHOTO_SIGS if k.startswith("derp_rephoto_
 REPHOTO_METHODS = {"MSSIM": 0, "NCC": 1}
 
 
-class Rephoto:
+class Rephoto(_Binding):
     """ctypes binding of include/derp_rephoto.h on a loaded library: ``Rephoto(load_cuda())`` for the product, or a
     path to another library exporting the same entry points (the CPU checker the tests build)."""
 
     def __init__(self, library):
-        if isinstance(library, Library):
-            self.path, self.lib = library.path, C.CDLL(library.path, mode=C.RTLD_LOCAL)
-        else:
-            if not os.path.exists(library):
-                raise FileNotFoundError(library)
-            self.path, self.lib = library, C.CDLL(library, mode=C.RTLD_LOCAL)
-        for name, (res, args) in _REPHOTO_SIGS.items():
-            fn = getattr(self.lib, name)  # AttributeError if a declared symbol is missing
-            fn.restype = res
-            fn.argtypes = args
-
-    def _check(self, rc):
-        if rc != 0:
-            raise DerpError(rc, self.lib.derp_last_error().decode())
+        self.path, self.lib = _bind(library, _REPHOTO_SIGS)
 
     def rephoto_cubemap(self, descs, disparities, colors_bgra, center, edge, want_color=True, want_disparity=False,
                         want_winners=False, device=0):
@@ -391,29 +392,27 @@ _CANOPY_SIGS = {
     "derp_canopy_render": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, _p(C.c_void_p), C.c_int, C.c_int, _p(C.c_void_p),
                                      C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float,
                                      C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "derp_canopy_snapshot_matrix": (C.c_int, [C.c_void_p] * 3 + [C.c_double, C.c_int, C.c_int, C.c_void_p]),
 }
-CANOPY_SYMBOLS = sorted(k for k in _CANOPY_SIGS if k.startswith("derp_canopy_")) + ["derp_canopy_snapshot_matrix"]
+CANOPY_SYMBOLS = sorted(k for k in _CANOPY_SIGS if k.startswith("derp_canopy_"))
 CANOPY_PROJECTIONS = {"cubemap": 0, "equirect": 1, "perspective": 2}
 CANOPY_SHADERS = {"on_screen": 0, "svd": 1}
 
 
-class Canopy:
-    """ctypes binding of include/derp_canopy.h's renderer on a loaded library: ``Canopy(load_cuda())`` for the product,
-    or a path to another library exporting derp_canopy_render (the CPU checker the tests build)."""
+class Canopy(_Binding):
+    """ctypes binding of include/derp_canopy.h on a loaded library: ``Canopy(load_cuda())`` for the product, or a path
+    to another library exporting derp_canopy_render (the CPU checker the tests build)."""
 
     def __init__(self, library):
-        path = library.path if isinstance(library, Library) else library
-        if not os.path.exists(path):
-            raise FileNotFoundError(path)
-        self.path, self.lib = path, C.CDLL(path, mode=C.RTLD_LOCAL)
-        for name, (res, args) in _CANOPY_SIGS.items():
-            fn = getattr(self.lib, name)  # AttributeError if a declared symbol is missing
-            fn.restype = res
-            fn.argtypes = args
+        self.path, self.lib = _bind(library, _CANOPY_SIGS, optional=("derp_canopy_snapshot_matrix",))
 
-    def _check(self, rc):
-        if rc != 0:
-            raise DerpError(rc, self.lib.derp_last_error().decode())
+    def snapshot_matrix(self, position, forward, up, horizontal_fov=90.0, width=3072, height=1536):
+        """SimpleMeshRenderer's snapshot clip matrix (computed on the host): float32 [4, 4]."""
+        vec = [np.ascontiguousarray(v, np.float32) for v in (position, forward, up)]
+        out = np.empty(16, np.float32)
+        self._check(self.lib.derp_canopy_snapshot_matrix(vec[0].ctypes.data, vec[1].ctypes.data, vec[2].ctypes.data,
+                                                         horizontal_fov, width, height, out.ctypes.data))
+        return out.reshape(4, 4)
 
     def render(self, descs, disparities, colors_bgra, position, projection="cubemap", size=(64, 64), matrix=None,
                ipd=0.0, alpha_blend=True, shader="svd", want_color=True, want_disparity=False, want_winners=False,
@@ -449,17 +448,10 @@ class Canopy:
 
 
 def snapshot_matrix(position, forward, up, horizontal_fov=90.0, width=3072, height=1536, library=None):
-    """SimpleMeshRenderer's snapshot clip matrix (derp_canopy_snapshot_matrix, computed on the host): float32 [4, 4]."""
-    lib = library.lib if library is not None else load_cuda().lib
-    f = lib.derp_canopy_snapshot_matrix
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p] * 3 + [C.c_double, C.c_int, C.c_int, C.c_void_p]
-    vec = [np.ascontiguousarray(v, np.float32) for v in (position, forward, up)]
-    out = np.empty(16, np.float32)
-    rc = f(vec[0].ctypes.data, vec[1].ctypes.data, vec[2].ctypes.data, horizontal_fov, width, height, out.ctypes.data)
-    if rc != 0:
-        raise DerpError(rc, lib.derp_last_error().decode())
-    return out.reshape(4, 4)
+    """SimpleMeshRenderer's snapshot clip matrix (derp_canopy_snapshot_matrix, computed on the host): float32 [4, 4].
+    `library`: a Library or Canopy binding, the product by default."""
+    canopy = library if isinstance(library, Canopy) else Canopy(library or load_cuda())
+    return canopy.snapshot_matrix(position, forward, up, horizontal_fov, width, height)
 
 
 class Context:
@@ -735,9 +727,13 @@ _SWEEP_SIGS = {
                                       C.c_void_p, C.c_int, C.c_void_p, C.c_int, _p(C.c_void_p)]),
     "derp_sweep_center_rig": (C.c_int, [_p(CameraDesc), C.c_int, C.c_int, _p(CameraDesc), C.c_void_p]),
     "derp_sweep_last_hits": (C.c_uint64, []),
+    "derp_sweep_crop_width": (C.c_int, [C.c_uint64, C.c_void_p, _p(C.c_uint64)]),
 }
-SWEEP_SYMBOLS = sorted(k for k in _SWEEP_SIGS if k.startswith("derp_sweep_")) + ["derp_sweep_crop_width"]
-SWEEP_TEST_HOOKS = ["derp_test_sweep_equirect_host", "derp_test_sweep_overlaps_host"]
+# derp_test_sweep_*_host: the same arguments as the entry point without the device
+_SWEEP_HOST_SIGS = {"derp_test_sweep_%s_host" % k: (C.c_int, _SWEEP_SIGS["derp_sweep_" + k][1][1:])
+                    for k in ("overlaps", "equirect")}
+SWEEP_SYMBOLS = sorted(k for k in _SWEEP_SIGS if k.startswith("derp_sweep_"))
+SWEEP_TEST_HOOKS = sorted(_SWEEP_HOST_SIGS)
 
 
 def rescaled_descs(descs, scale):
@@ -759,31 +755,15 @@ def rescaled_descs(descs, scale):
     return out
 
 
-class SweepView:
+class SweepView(_Binding):
     """ctypes binding of include/derp_sweepview.h on a loaded library: ``SweepView(load_cuda())`` for the product, or a
     path to a library exporting some of the same entry points (the CPU checkers the tests build).  ``host=True`` runs
     the product's DERP_HD per-pixel code on the host (derp_test_sweep_*_host)."""
 
     def __init__(self, library, host=False):
-        path = library.path if isinstance(library, Library) else library
-        if not os.path.exists(path):
-            raise FileNotFoundError(path)
-        self.path, self.lib, self.host = path, C.CDLL(path, mode=C.RTLD_LOCAL), host
-        for name, (res, args) in _SWEEP_SIGS.items():
-            fn = getattr(self.lib, name, None)
-            if fn is not None:
-                fn.restype = res
-                fn.argtypes = args
-        if host:
-            for name, sig in (("derp_test_sweep_overlaps_host", "derp_sweep_overlaps"),
-                              ("derp_test_sweep_equirect_host", "derp_sweep_equirect")):
-                fn = getattr(self.lib, name)
-                fn.restype = C.c_int
-                fn.argtypes = _SWEEP_SIGS[sig][1][1:]  # the same arguments without the device
-
-    def _check(self, rc):
-        if rc != 0:
-            raise DerpError(rc, self.lib.derp_last_error().decode())
+        sigs = dict(_SWEEP_SIGS, **_SWEEP_HOST_SIGS) if host else _SWEEP_SIGS
+        self.path, self.lib = _bind(library, sigs, optional=_SWEEP_SIGS)
+        self.host = host
 
     @staticmethod
     def _images(images):
@@ -816,12 +796,9 @@ class SweepView:
         return out
 
     def crop_width(self, height, box):
-        f = self.lib.derp_sweep_crop_width
-        f.restype = C.c_int
-        f.argtypes = [C.c_uint64, C.c_void_p, _p(C.c_uint64)]
         b = np.ascontiguousarray(box, np.float64)
         w = C.c_uint64()
-        self._check(f(height, b.ctypes.data, C.byref(w)))
+        self._check(self.lib.derp_sweep_crop_width(height, b.ctypes.data, C.byref(w)))
         return w.value
 
     def equirect(self, descs, images, height, depths, bounds=None, black_bg=False, center=-1, widths=None, device=0):

@@ -1,72 +1,28 @@
 // libderp_b200.so — the product: C ABI of include/derp_b200.h implemented with hand-written
 // sm_90a CUDA kernels (derp_kernels.cuh).  No CPU fallback: every entry point that computes
-// needs a CUDA device and fails with DERP_ECUDA otherwise.
+// needs a CUDA device and fails with DERP_ECUDA otherwise.  This file holds the depth context (DerpCtx) and the
+// stand-alone depth stages; derp_convert.cu, derp_canopy.cu and derp_sweepview.cu hold the other entry points.
 //
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see Makefile).
-#include <cuda_runtime.h>
-
-#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <memory>
-#include <string>
-#include <vector>
 
-#include "../../include/derp_b200.h"
+#include "derp_host.cuh"
 #include "derp_kernels.cuh"
 #include "derp_refine.cuh"
-#include "derp_mesh.cuh"
-#include "derp_simplify.h"
-#include "derp_bc7.cuh"
-#include "derp_rephoto.cuh"
-#include "derp_sweepview.cuh"
-#include "../../include/derp_rephoto.h"
-#include "../../include/derp_canopy.h"
-#include "../../include/derp_sweepview.h"
 
 using namespace derp;
 
-namespace {
-
 thread_local std::string g_err;
 
-int fail(int code, const std::string& msg) {
-  g_err = msg;
-  return code;
-}
+static_assert(kBlock2X == kBlockX && kBlock2Y == kBlockY, "grid2 / block2 must launch the kernels' CTA");
 
-#define CU(call)                                                                                     \
-  do {                                                                                               \
-    cudaError_t e_ = (call);                                                                         \
-    if (e_ != cudaSuccess)                                                                           \
-      return fail(DERP_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_) + " (" + __FILE__ + ":" + \
-                                  std::to_string(__LINE__) + ")");                                   \
-  } while (0)
+namespace {
 
-template <typename T>
-struct DevBuf {
-  T* p = nullptr;
-  size_t n = 0;
-  ~DevBuf() { release(); }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    n = 0;
-  }
-  cudaError_t ensure(size_t count) {
-    if (count <= n && p) return cudaSuccess;
-    release();
-    cudaError_t e = cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) n = count;
-    return e;
-  }
-};
-
-inline dim3 grid2(int W, int H, int z = 1) { return dim3((W + kBlockX - 1) / kBlockX, (H + kBlockY - 1) / kBlockY, z); }
-inline dim3 block2() { return dim3(kBlockX, kBlockY, 1); }
 // Grid of the kernels that walk the active-pixel list: one CTA per kPatchThreads list slots of the largest
 // possible list (its length is only known on the device); CTAs past the end exit before staging anything.  A
 // capped grid with more loop trips per CTA is not faster.
@@ -78,7 +34,6 @@ inline size_t bilateralSmem(int radius) {  // float4 tile + mask bytes of bilate
   const size_t cells = (size_t)(kBlockX + 2 * radius) * (kBlockY + 2 * radius);
   return cells * sizeof(float4) + ((cells + 15) / 16) * 16;
 }
-inline unsigned grid1(size_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
 
 // OpenCV's float bicubic table (imgwarp.cpp: interpolateCubic A=-0.75, initInterTab2D, INTER_TAB_SIZE 32)
 void buildBicubicTable(std::vector<float>& tab) {
@@ -116,10 +71,6 @@ void lanczosTaps(float x, float* c) {
   sum = 1.f / sum;
   for (int i = 0; i < 8; ++i) c[i] *= sum;
 }
-int floorD(double v) {
-  int i = (int)v;
-  return i - (i > v);
-}
 void lanczosAxis(int sn, int dn, std::vector<int>& ofs, std::vector<float>& taps) {
   const double inv = (double)dn / sn, scale = 1. / inv;
   ofs.resize(dn);
@@ -131,11 +82,6 @@ void lanczosAxis(int sn, int dn, std::vector<int>& ofs, std::vector<float>& taps
     ofs[d] = s;
     lanczosTaps(f, &taps[(size_t)d * 8]);
   }
-}
-void nearestAxis(int sn, int dn, std::vector<int>& ofs) {
-  const double inv = (double)dn / sn, ifx = 1. / inv;
-  ofs.resize(dn);
-  for (int d = 0; d < dn; ++d) ofs[d] = std::min(floorD(d * ifx), sn - 1);
 }
 // UpsampleDisparityLib.cpp:27-52: clock-wise outward spiral of diameter w
 void spiralOffsets(int w, std::vector<short2>& locs) {
@@ -1058,19 +1004,12 @@ int derp_gather_disparities(DerpCtx* c, const float* const* planes) {
       CU(cudaMemcpyAsync(to, c->dDisp.p + (size_t)ownDst[s] * n, b, cudaMemcpyDeviceToDevice, c->stream));
       continue;
     }
-    cudaPointerAttributes at{};
-    CU(cudaPointerGetAttributes(&at, from));
-    if (at.type == cudaMemoryTypeDevice && at.device != c->device) {
+    const int peer = deviceOf(from);
+    if (peer >= 0 && peer != c->device) {
       // a peer context's plane: device-to-device over NVLink (the runtime stages through the host if the two
       // devices have no peer path)
-      int can = 0;
-      CU(cudaDeviceCanAccessPeer(&can, c->device, at.device));
-      if (can) {
-        const cudaError_t e = cudaDeviceEnablePeerAccess(at.device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CU(e);
-        (void)cudaGetLastError();
-      }
-      CU(cudaMemcpyPeerAsync(to, c->device, from, at.device, b, c->stream));
+      if ((rc = enablePeer(c->device, peer))) return rc;
+      CU(cudaMemcpyPeerAsync(to, c->device, from, peer, b, c->stream));
     } else {
       CU(cudaMemcpyAsync(to, from, b, cudaMemcpyDefault, c->stream));
     }
@@ -1234,18 +1173,10 @@ int derp_upsample_from(DerpCtx* c, int dst, const float* coarse, int coarse_w, i
   int rc = checkDst(c, dst, "derp_upsample_from", false);
   if (rc) return rc;
   const size_t nc = (size_t)coarse_w * coarse_h;
-  cudaPointerAttributes a;
-  const bool onDevice = cudaPointerGetAttributes(&a, coarse) == cudaSuccess &&
-      (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged);
-  cudaGetLastError();
-  const float* dCoarse = coarse;
-  if (!onDevice) {  // host plane (the PFM a caller read back): staged once into a context buffer
-    CU(c->dUpCoarse.ensure(nc));
-    CU(cudaMemcpyAsync(c->dUpCoarse.p, coarse, nc * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    dCoarse = c->dUpCoarse.p;
-  }
+  const float* dCoarse = coarse;  // a host plane (the PFM a caller read back) is staged into a context buffer
+  if ((rc = stageIn(dCoarse, nc, c->dUpCoarse, alignof(float), c->stream))) return rc;
   rc = upsampleIntoLevel(c, dst, dCoarse, coarse_w, coarse_h, coarse_mask, fine_mask, "derp_upsample_from");
-  if (rc == DERP_OK && !onDevice) CU(cudaStreamSynchronize(c->stream));  // the caller's host plane may be reused on return
+  if (rc == DERP_OK && dCoarse != coarse) CU(cudaStreamSynchronize(c->stream));  // the caller's plane may be reused on return
   return rc;
 }
 
@@ -1304,27 +1235,11 @@ int derp_downscale_area(int device, const uint16_t* src, int src_w, int src_h, u
   CU(cudaSetDevice(device));
   const size_t ns = (size_t)src_w * src_h * 3, nd = (size_t)dst_w * dst_h * 3;
   // device-resident images are used in place; host images are staged
-  auto onDevice = [](const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-      cudaGetLastError();
-      return false;
-    }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-  };
-  const bool srcDev = onDevice(src), dstDev = onDevice(dst);
   DevBuf<uint16_t> dS, dD;
   const uint16_t* sp = src;
   uint16_t* dp = dst;
-  if (!srcDev) {
-    CU(dS.ensure(ns));
-    CU(cudaMemcpy(dS.p, src, ns * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    sp = dS.p;
-  }
-  if (!dstDev) {
-    CU(dD.ensure(nd));
-    dp = dD.p;
-  }
+  int rc = stageIn(sp, ns, dS);
+  if (rc || (rc = outBuffer(dp, nd, dD))) return rc;
   const double sx = (double)src_w / dst_w, sy = (double)src_h / dst_h;
   const int kx = (int)std::floor(sx + 0.5), ky = (int)std::floor(sy + 0.5);
   const dim3 grid((dst_w * 3 + 255) / 256, dst_h);
@@ -1353,8 +1268,8 @@ int derp_downscale_area(int device, const uint16_t* src, int src_w, int src_h, u
     CU(cudaDeviceSynchronize());  // tables are freed on return
   }
   CU(cudaGetLastError());
-  if (!dstDev) CU(cudaMemcpy(dst, dD.p, nd * sizeof(uint16_t), cudaMemcpyDeviceToHost));
-  else if (!srcDev) CU(cudaDeviceSynchronize());  // the staged source is freed on return
+  if (dp != dst) return stageOut(dst, dp, nd);
+  if (sp != src) CU(cudaDeviceSynchronize());  // the staged source is freed on return
   return DERP_OK;
 }
 
@@ -1375,15 +1290,9 @@ int derp_device_copy(int device, void* dst, const void* src, size_t bytes) {
   CU(cudaSetDevice(device));
   // a source (or destination) on another GPU: make sure the direct NVLink path is enabled
   for (const void* p : {src, (const void*)dst}) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device != device) {
-      int can = 0;
-      if (cudaDeviceCanAccessPeer(&can, device, a.device) == cudaSuccess && can) {
-        const cudaError_t e = cudaDeviceEnablePeerAccess(a.device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fail(DERP_ECUDA, cudaGetErrorString(e));
-      }
-    }
-    cudaGetLastError();
+    const int other = deviceOf(p);
+    if (other >= 0 && other != device)
+      if (int rc = enablePeer(device, other)) return rc;
   }
   CU(cudaMemcpy(dst, src, bytes, cudaMemcpyDefault));
   return DERP_OK;
@@ -1423,204 +1332,6 @@ int derp_foreground_mask(int device, const uint16_t* templ, const uint16_t* fram
   CU(cudaGetLastError());
   CU(cudaMemcpy(mask, dM.p, n, cudaMemcpyDefault));
   return DERP_OK;
-}
-
-// cv::resize(depth, depth, Size(), s, s, INTER_NEAREST) (ConvertToBinary.cpp:153-156): dsize = cvRound(size * s),
-// source index = min(floor(d * (1 / s)), size - 1) (resize.cpp resizeNN with the caller's scale factors)
-static void meshAxis(int sn, double scale, std::vector<int>& ofs) {
-  if (!(scale < 1)) {
-    ofs.resize(sn);
-    for (int d = 0; d < sn; ++d) ofs[d] = d;
-    return;
-  }
-  const int dn = (int)std::nearbyint(sn * scale);
-  const double ifx = 1. / scale;
-  ofs.resize(std::max(dn, 0));
-  for (int d = 0; d < dn; ++d) ofs[d] = std::min(floorD(d * ifx), sn - 1);
-}
-
-int derp_camera_mesh_size(int width, int height, double depth_scale, int* mesh_width, int* mesh_height) {
-  if (width < 1 || height < 1 || !(depth_scale > 0) || depth_scale > 1 || !mesh_width || !mesh_height)
-    return fail(DERP_EINVAL, "derp_camera_mesh_size: bad arguments (depth_scale in (0, 1], ConvertToBinary.cpp:348)");
-  *mesh_width = depth_scale < 1 ? (int)std::nearbyint(width * depth_scale) : width;
-  *mesh_height = depth_scale < 1 ? (int)std::nearbyint(height * depth_scale) : height;
-  return DERP_OK;
-}
-
-static int cameraMesh(int device, const float* disparity, int width, int height, double depth_scale, double resolution_x,
-                      double resolution_y, double scalar_focal, float tear_ratio, const uint8_t* foreground_mask,
-                      int mask_width, int mask_height, int triangles, float* vertexes, uint32_t* faces,
-                      uint64_t* num_vertexes, uint64_t* num_faces) {
-  int W = 0, H = 0;
-  int rc = derp_camera_mesh_size(width, height, depth_scale, &W, &H);
-  if (rc) return rc;
-  if (!disparity || !vertexes || !faces || !num_vertexes || !num_faces || W < 1 || H < 1 ||
-      (foreground_mask && (mask_width < 1 || mask_height < 1)))
-    return fail(DERP_EINVAL, "derp_camera_mesh: bad arguments");
-  CU(cudaSetDevice(device));
-  const size_t n = (size_t)W * H, nsrc = (size_t)width * height;
-  if (n >= (1ull << 31)) return fail(DERP_EINVAL, "derp_camera_mesh: grid too large for 32-bit indexes");
-  std::vector<int> ofs, tmp;
-  meshAxis(width, depth_scale, ofs);
-  meshAxis(height, depth_scale, tmp);
-  ofs.insert(ofs.end(), tmp.begin(), tmp.end());
-  if (foreground_mask) {  // cv::resize(mask, mask, depth.size(), 0, 0, INTER_NEAREST), ConvertToBinary.cpp:171-174
-    nearestAxis(mask_width, W, tmp);
-    ofs.insert(ofs.end(), tmp.begin(), tmp.end());
-    nearestAxis(mask_height, H, tmp);
-    ofs.insert(ofs.end(), tmp.begin(), tmp.end());
-  }
-  // grow-only scratch per host thread (the app converts one (frame, camera) after the other on each GPU worker thread)
-  struct MeshScratch {
-    DevBuf<float> dDisp, dVtx;
-    DevBuf<double> dVtx64;
-    DevBuf<int> dOfs;
-    DevBuf<uint8_t> dFg, dQuad, dUsed;
-    DevBuf<unsigned> dTiles, dIndex, dFaces;
-    DevBuf<unsigned long long> dTotals;
-    int device = -1;
-  };
-  static thread_local MeshScratch sc;
-  if (sc.device != device) {  // the thread moved to another GPU: the old buffers belong to the old device
-    if (sc.device >= 0) {
-      cudaSetDevice(sc.device);
-      sc.dDisp.release();
-      sc.dVtx.release();
-      sc.dVtx64.release();
-      sc.dOfs.release();
-      sc.dFg.release();
-      sc.dQuad.release();
-      sc.dUsed.release();
-      sc.dTiles.release();
-      sc.dIndex.release();
-      sc.dFaces.release();
-      sc.dTotals.release();
-      CU(cudaSetDevice(device));
-    }
-    sc.device = device;
-  }
-  DevBuf<float>&dDisp = sc.dDisp, &dVtx = sc.dVtx;
-  DevBuf<int>& dOfs = sc.dOfs;
-  DevBuf<uint8_t>&dFg = sc.dFg, &dQuad = sc.dQuad, &dUsed = sc.dUsed;
-  DevBuf<unsigned>&dTiles = sc.dTiles, &dIndex = sc.dIndex, &dFaces = sc.dFaces;
-  DevBuf<unsigned long long>& dTotals = sc.dTotals;
-  const float* disp = disparity;
-  const uint8_t* fg = foreground_mask;
-  cudaPointerAttributes at{};
-  if (cudaPointerGetAttributes(&at, disparity) != cudaSuccess || at.type != cudaMemoryTypeDevice) {
-    (void)cudaGetLastError();
-    CU(dDisp.ensure(nsrc));
-    CU(cudaMemcpy(dDisp.p, disparity, nsrc * sizeof(float), cudaMemcpyDefault));
-    disp = dDisp.p;
-  }
-  if (fg && (cudaPointerGetAttributes(&at, fg) != cudaSuccess || at.type != cudaMemoryTypeDevice)) {
-    (void)cudaGetLastError();
-    CU(dFg.ensure((size_t)mask_width * mask_height));
-    CU(cudaMemcpy(dFg.p, fg, (size_t)mask_width * mask_height, cudaMemcpyDefault));
-    fg = dFg.p;
-  }
-  const int tiles = (int)((n + kScanTile - 1) / kScanTile);
-  CU(dOfs.ensure(ofs.size()));
-  CU(cudaMemcpy(dOfs.p, ofs.data(), ofs.size() * sizeof(int), cudaMemcpyHostToDevice));
-  CU(dQuad.ensure(n));
-  CU(dUsed.ensure(n));
-  CU(dTiles.ensure(2 * (size_t)tiles));
-  CU(dIndex.ensure(n));
-  CU(dTotals.ensure(2));
-  CU(cudaMemset(dUsed.p, 0, n));
-  MeshGrid g;
-  g.W = W;
-  g.H = H;
-  g.srcW = width;
-  g.disp = disp;
-  g.xofs = dOfs.p;
-  g.yofs = dOfs.p + W;
-  g.fg = fg;
-  g.fgW = mask_width;
-  g.fgx = dOfs.p + W + H;
-  g.fgy = dOfs.p + 2 * (size_t)W + H;
-  g.stepX = resolution_x / W;
-  g.stepY = resolution_y / H;
-  g.scale = scalar_focal * 1.0;  // kRadius = 1 (MeshUtil.h:316)
-  g.tearRatio = tear_ratio;
-  g.floorZ = 0;
-  meshQuadKernel<<<grid2(W, H), block2()>>>(g, dQuad.p, dUsed.p);
-  meshTileCountKernel<<<tiles, kScanThreads>>>(n, dQuad.p, dUsed.p, dTiles.p, dTiles.p + tiles);
-  meshTileScanKernel<<<1, kScanThreads>>>(tiles, dTiles.p, dTiles.p + tiles, dTotals.p);
-  CU(cudaGetLastError());
-  unsigned long long totals[2] = {0, 0};
-  CU(cudaMemcpy(totals, dTotals.p, sizeof(totals), cudaMemcpyDeviceToHost));
-  if (triangles > 0 && totals[0] > (unsigned long long)triangles) {
-    // Simplification (ConvertToBinary.cpp:186-203): the mesh in double precision goes to the host, where the strictly
-    // sequential edge-contraction sweeps run (derp_simplify.h), like MeshSimplifier with kThreads = 1 in the reference.
-    DevBuf<double>& dVtx64 = sc.dVtx64;
-    CU(dVtx64.ensure(std::max<size_t>(1, totals[1] * 3)));
-    CU(dFaces.ensure(std::max<size_t>(1, totals[0] * 3)));
-    g.floorZ = 0;  // the simplifier works on the raw values; the floor is applied to its output below
-    meshEmitVertexesKernel<double><<<tiles, kScanThreads>>>(g, dUsed.p, dTiles.p + tiles, dIndex.p, dVtx64.p);
-    meshEmitFacesKernel<<<tiles, kScanThreads>>>(W, n, dQuad.p, dTiles.p, dIndex.p, dFaces.p);
-    CU(cudaGetLastError());
-    std::vector<double> hv(totals[1] * 3);
-    std::vector<uint32_t> hf(totals[0] * 3);
-    CU(cudaMemcpy(hv.data(), dVtx64.p, hv.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(hf.data(), dFaces.p, hf.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    simplify::Mesh mesh(hv.data(), totals[1], hf.data(), totals[0]);
-    mesh.run(triangles, 0.2f, false);  // kStrictness, kRemoveBoundaryEdges (ConvertToBinary.cpp:193-195)
-    std::vector<float> ov(mesh.verts.size() * 3);
-    std::vector<uint32_t> of(mesh.faces.size() * 3);
-    for (size_t i = 0; i < mesh.verts.size(); ++i) {
-      const simplify::V3& p = mesh.verts[i].p;
-      ov[3 * i] = (float)p.x;
-      ov[3 * i + 1] = (float)p.y;
-      ov[3 * i + 2] = (float)(p.z < 0 ? (double)FLT_MIN : p.z);  // ConvertToBinary.cpp:199-203
-    }
-    for (size_t i = 0; i < mesh.faces.size(); ++i)
-      for (int j = 0; j < 3; ++j) of[3 * i + j] = (uint32_t)mesh.faces[i].v[j];
-    CU(cudaMemcpy(vertexes, ov.data(), ov.size() * sizeof(float), cudaMemcpyDefault));
-    CU(cudaMemcpy(faces, of.data(), of.size() * sizeof(uint32_t), cudaMemcpyDefault));
-    *num_vertexes = mesh.verts.size();
-    *num_faces = mesh.faces.size();
-    return DERP_OK;
-  }
-  g.floorZ = triangles > 0;  // the reference applies it after the (here: no-op) simplification
-  // outputs: written in place when the caller's buffers are device memory, else staged
-  float* vtx = vertexes;
-  uint32_t* fac = faces;
-  if (cudaPointerGetAttributes(&at, vertexes) != cudaSuccess || at.type != cudaMemoryTypeDevice) {
-    (void)cudaGetLastError();
-    CU(dVtx.ensure(std::max<size_t>(1, totals[1] * 3)));
-    vtx = dVtx.p;
-  }
-  if (cudaPointerGetAttributes(&at, faces) != cudaSuccess || at.type != cudaMemoryTypeDevice) {
-    (void)cudaGetLastError();
-    CU(dFaces.ensure(std::max<size_t>(1, totals[0] * 3)));
-    fac = dFaces.p;
-  }
-  meshEmitVertexesKernel<float><<<tiles, kScanThreads>>>(g, dUsed.p, dTiles.p + tiles, dIndex.p, vtx);
-  meshEmitFacesKernel<<<tiles, kScanThreads>>>(W, n, dQuad.p, dTiles.p, dIndex.p, fac);
-  CU(cudaGetLastError());
-  if (vtx != vertexes) CU(cudaMemcpy(vertexes, vtx, totals[1] * 3 * sizeof(float), cudaMemcpyDefault));
-  if (fac != faces) CU(cudaMemcpy(faces, fac, totals[0] * 3 * sizeof(uint32_t), cudaMemcpyDefault));
-  CU(cudaDeviceSynchronize());
-  *num_faces = totals[0];
-  *num_vertexes = totals[1];
-  return DERP_OK;
-}
-
-int derp_camera_mesh(int device, const float* disparity, int width, int height, double depth_scale, double resolution_x,
-                     double resolution_y, double scalar_focal, float tear_ratio, const uint8_t* foreground_mask,
-                     int mask_width, int mask_height, float* vertexes, uint32_t* faces, uint64_t* num_vertexes,
-                     uint64_t* num_faces) {
-  return cameraMesh(device, disparity, width, height, depth_scale, resolution_x, resolution_y, scalar_focal, tear_ratio,
-                    foreground_mask, mask_width, mask_height, 0, vertexes, faces, num_vertexes, num_faces);
-}
-
-int derp_camera_mesh_simplified(int device, const float* disparity, int width, int height, double depth_scale,
-                                double resolution_x, double resolution_y, double scalar_focal, float tear_ratio,
-                                const uint8_t* foreground_mask, int mask_width, int mask_height, int triangles,
-                                float* vertexes, uint32_t* faces, uint64_t* num_vertexes, uint64_t* num_faces) {
-  return cameraMesh(device, disparity, width, height, depth_scale, resolution_x, resolution_y, scalar_focal, tear_ratio,
-                    foreground_mask, mask_width, mask_height, triangles, vertexes, faces, num_vertexes, num_faces);
 }
 
 int derp_upsample_disparity(int device, const DerpCameraDesc* cam, const float* coarse, int coarse_w, int coarse_h,
@@ -1910,21 +1621,8 @@ int derp_temporal_filter(int device, int width, int height, int num_frames, cons
     DevBuf<uint2> dG;
     DevBuf<float> dD, dOut;
     DevBuf<uint8_t> dM, dStage;
-    int device = -1;
   };
   static thread_local Scratch sc;
-  if (sc.device != device) {  // the thread moved to another GPU: the old buffers belong to the old device
-    if (sc.device >= 0) {
-      cudaSetDevice(sc.device);
-      sc.dG.release();
-      sc.dD.release();
-      sc.dOut.release();
-      sc.dM.release();
-      sc.dStage.release();
-      CU(cudaSetDevice(device));
-    }
-    sc.device = device;
-  }
   DevBuf<uint2>& dG = sc.dG;
   DevBuf<float>&dD = sc.dD, &dOut = sc.dOut;
   DevBuf<uint8_t>&dM = sc.dM, &dStage = sc.dStage;
@@ -1990,359 +1688,6 @@ int derp_joint_bilateral_f32(int device, int width, int height, const float* ima
   return DERP_OK;
 }
 
-
-// ---- BC7 colour (ConvertToBinary's default colour format) ----
-static int bc7Launch(int device, const void* src, size_t srcBytes, int mode, int channels, int width, int height,
-                     const uint8_t* lutHost, size_t lutBytes, uint8_t* blocks) {
-  CU(cudaSetDevice(device));
-  const size_t outBytes = (size_t)width * height;
-  DevBuf<uint8_t> dSrc, dOut, dLut;
-  const void* s = src;
-  cudaPointerAttributes at{};
-  if (cudaPointerGetAttributes(&at, src) != cudaSuccess || at.type != cudaMemoryTypeDevice) {
-    (void)cudaGetLastError();
-    CU(dSrc.ensure(srcBytes));
-    CU(cudaMemcpy(dSrc.p, src, srcBytes, cudaMemcpyDefault));
-    s = dSrc.p;
-  }
-  uint8_t* o = blocks;
-  const bool outOnDevice = cudaPointerGetAttributes(&at, blocks) == cudaSuccess && at.type == cudaMemoryTypeDevice;
-  if (!outOnDevice) {
-    (void)cudaGetLastError();
-    CU(dOut.ensure(outBytes));
-    o = dOut.p;
-  }
-  CU(cudaMemset(o, 0, outBytes));  // the reference's output vector starts zeroed; partial edge blocks are never written
-  const int bx = width / 4, by = height / 4;
-  if (bx > 0 && by > 0) {
-    const unsigned grid = (unsigned)(((size_t)bx * by + derp::bc7::kBc7Threads - 1) / derp::bc7::kBc7Threads);
-    if (mode == 0) {
-      derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(derp::bc7::Rgba8Source{(const uint8_t*)s, width}, width, bx, by, o);
-    } else {
-      CU(dLut.ensure(lutBytes));
-      CU(cudaMemcpy(dLut.p, lutHost, lutBytes, cudaMemcpyHostToDevice));
-      if (mode == 8)
-        derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(
-            derp::bc7::BgrSource<uint8_t>{(const uint8_t*)s, width, channels, dLut.p}, width, bx, by, o);
-      else
-        derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(
-            derp::bc7::BgrSource<uint16_t>{(const uint16_t*)s, width, channels, dLut.p}, width, bx, by, o);
-    }
-    CU(cudaGetLastError());
-  }
-  if (!outOnDevice) CU(cudaMemcpy(blocks, o, outBytes, cudaMemcpyDeviceToHost));
-  else CU(cudaDeviceSynchronize());
-  return DERP_OK;
-}
-
-int derp_bc7_compress(int device, const uint8_t* rgba, int width, int height, uint8_t* blocks) {
-  if (!rgba || !blocks || width < 1 || height < 1) return fail(DERP_EINVAL, "derp_bc7_compress: bad arguments");
-  return bc7Launch(device, rgba, (size_t)width * height * 4, 0, 4, width, height, nullptr, 0, blocks);
-}
-
-int derp_bc7_compress_image(int device, const void* pixels, int bits_per_channel, int channels, int width, int height,
-                            float gamma, uint8_t* blocks) {
-  if (!pixels || !blocks || width < 1 || height < 1 || (bits_per_channel != 8 && bits_per_channel != 16) ||
-      (channels != 3 && channels != 4))
-    return fail(DERP_EINVAL, "derp_bc7_compress_image: 8 or 16 bits per channel, 3 (BGR) or 4 (BGRA) channels");
-  std::vector<uint8_t> lut((size_t)1 << bits_per_channel);
-  derp::bc7::gammaTable(bits_per_channel, gamma, lut.data());
-  return bc7Launch(device, pixels, (size_t)width * height * channels * (bits_per_channel / 8), bits_per_channel, channels,
-                   width, height, lut.data(), lut.size(), blocks);
-}
-
-}  // extern "C"
-
-// ---- rephotography (derp_rephoto.cuh) ----------------------------------------------------------------
-// Grow-only scratch per host thread, like the camera mesh: the app renders four cubemaps and one score per camera.
-namespace {
-struct RephotoScratch {
-  DevBuf<float> disp, bgra, vtx, out, f32, mats, trig, eq;
-  DevBuf<ushort4> texC, texD;
-  DevBuf<unsigned long long> keys;
-  DevBuf<float4> accC, accD;
-  DevBuf<int> flags;
-  DevBuf<int32_t> win;
-  DevBuf<uint8_t> mask;
-  DevBuf<double> partial;
-  int device = -1;
-  void release() {
-    disp.release(); bgra.release(); vtx.release(); out.release(); f32.release(); mats.release(); trig.release();
-    eq.release(); texC.release(); texD.release();
-    keys.release(); accC.release(); accD.release(); flags.release(); win.release(); mask.release(); partial.release();
-  }
-};
-thread_local RephotoScratch g_rephoto;
-
-int rephotoScratch(int device) {
-  RephotoScratch& s = g_rephoto;
-  if (s.device != device) {
-    if (s.device >= 0) {
-      cudaSetDevice(s.device);
-      s.release();
-    }
-    s.device = device;
-  }
-  CU(cudaSetDevice(device));
-  return DERP_OK;
-}
-
-// CanopyScene::cubemap / equirect / render (derp_canopy.h) in every mode; rephotography is the cubemap, ipd 0,
-// alpha-blended, on-screen case with NaN set to 0.  When the colour and the disparity colour are both wanted at one
-// texture size, one raster serves both; otherwise each scene is a pass of its own (the alpha test and the LOD depend on
-// the texture's size).
-int canopyRender(const char* who, int device, const DerpCameraDesc* cams, int num_cams, const float* const* disparities,
-                 int mw, int mh, const float* const* colors_bgra, int cw, int ch, int projection, const float* position,
-                 const float* matrix, int outW, int outH, float ipd, int alphaBlend, int shader, bool zeroNan,
-                 float* out_color, float* out_disparity, int32_t* winners) {
-  using namespace derp::rephoto;
-  const std::string name(who);
-  if (!cams || num_cams < 0 || (num_cams > 0 && !disparities) || mw < 2 || mh < 2 || !position ||
-      (!out_color && !out_disparity) || (out_color && num_cams > 0 && !colors_bgra) || (out_color && (cw < 1 || ch < 1)))
-    return fail(DERP_EINVAL, name + ": bad arguments");
-  if (shader != DERP_CANOPY_ON_SCREEN && shader != DERP_CANOPY_SVD)
-    return fail(DERP_EINVAL, name + ": shader must be DERP_CANOPY_ON_SCREEN or DERP_CANOPY_SVD");
-  int views, W, H;  // the raster: `views` viewports of W x H
-  if (projection == DERP_CANOPY_CUBEMAP || projection == DERP_CANOPY_EQUIRECT) {
-    const bool ok = projection == DERP_CANOPY_CUBEMAP ? outW == outH : outW == 2 * outH;
-    if (!ok || outH < 2) return fail(DERP_EINVAL, name + ": bad output size for the projection");
-    views = kFaces;
-    W = H = outH;
-  } else if (projection == DERP_CANOPY_PERSPECTIVE) {
-    if (!matrix || outW < 1 || outH < 1) return fail(DERP_EINVAL, name + ": perspective needs a matrix and a size");
-    views = 1;
-    W = outW;
-    H = outH;
-  } else {
-    return fail(DERP_EINVAL, name + ": unknown projection");
-  }
-  if ((long long)mw * mh >= (1ll << 30) || (out_color && (long long)cw * ch >= (1ll << 30)) ||
-      (long long)W * H * views >= (1ll << 31))
-    return fail(DERP_EINVAL, name + ": image or output too large");
-  std::vector<DevCamera> dcMesh(num_cams), dcTex(num_cams);
-  for (int i = 0; i < num_cams; ++i) {
-    DevCamera c;
-    if (!host::makeCamera(cams[i], &c)) return fail(DERP_EINVAL, name + ": invalid camera " + std::to_string(i));
-    dcMesh[i] = host::rescaled(c, mw, mh);  // camera.rescale({disparity.cols, disparity.rows})
-    if (out_color) dcTex[i] = host::rescaled(c, cw, ch);  // alphaFov: camera.rescale({color.cols, color.rows})
-  }
-  std::vector<float> mats(16 * views);
-  if (views == kFaces) {
-    FaceMats fm;
-    faceMatrices(position, &fm);
-    for (int f = 0; f < kFaces; ++f) std::memcpy(&mats[16 * f], fm.m[f], 16 * sizeof(float));
-  } else {
-    std::memcpy(mats.data(), matrix, 16 * sizeof(float));
-  }
-  struct Pass {
-    bool color, disp;
-  };
-  std::vector<Pass> passes;
-  if (out_color && out_disparity && cw == mw && ch == mh) {
-    passes.push_back({true, true});
-  } else {
-    if (out_color) passes.push_back({true, false});
-    if (out_disparity) passes.push_back({false, true});
-  }
-  int rc = rephotoScratch(device);
-  if (rc) return rc;
-  RephotoScratch& s = g_rephoto;
-  const size_t n = (size_t)mw * mh, nc = out_color ? (size_t)cw * ch : 0;
-  const size_t pixels = (size_t)views * W * H;
-  CU(s.disp.ensure(n));
-  CU(s.vtx.ensure(n * 3));
-  CU(s.keys.ensure(pixels));
-  CU(s.flags.ensure(1));
-  CU(s.mats.ensure(mats.size()));
-  CU(cudaMemcpy(s.mats.p, mats.data(), mats.size() * sizeof(float), cudaMemcpyHostToDevice));
-  if (out_color) {
-    CU(s.bgra.ensure(nc * 4));
-    CU(s.accC.ensure(pixels));
-    CU(cudaMemset(s.accC.p, 0, pixels * sizeof(float4)));
-  }
-  if (out_disparity) {
-    CU(s.accD.ensure(pixels));
-    CU(cudaMemset(s.accD.p, 0, pixels * sizeof(float4)));
-  }
-  if (winners) CU(s.win.ensure(pixels * std::max(num_cams, 1)));
-  CU(s.out.ensure(pixels * 4));
-  const int prims = (mw - 1) * (mh - 1) * 2;
-  for (size_t pi = 0; pi < passes.size(); ++pi) {
-    const Pass& ps = passes[pi];
-    const int tw = ps.color ? cw : mw, th = ps.color ? ch : mh;
-    int levels = 1;
-    while ((tw >> levels) > 0 || (th >> levels) > 0) ++levels;
-    if (levels > kMaxLevels) return fail(DERP_EINVAL, name + ": image too large");
-    Canopy cv{};
-    cv.mw = mw;
-    cv.mh = mh;
-    cv.levels = levels;
-    cv.svd = shader == DERP_CANOPY_SVD;
-    cv.alphaBlend = alphaBlend != 0;
-    long long texels = 0;
-    for (int l = 0; l < levels; ++l) {
-      cv.lw[l] = std::max(1, tw >> l);
-      cv.lh[l] = std::max(1, th >> l);
-      cv.lofs[l] = texels;
-      texels += (long long)cv.lw[l] * cv.lh[l];
-    }
-    if (ps.color) CU(s.texC.ensure(texels));
-    if (ps.disp) CU(s.texD.ensure(texels));
-    ushort4* texC = ps.color ? s.texC.p : nullptr;
-    ushort4* texD = ps.disp ? s.texD.p : nullptr;
-    cv.vtx = s.vtx.p;
-    cv.tex[0] = texC;
-    cv.tex[1] = texD;
-    int32_t* win = winners && pi == 0 ? s.win.p : nullptr;
-    const bool ownGrid = ps.color && (cw != mw || ch != mh);  // the colour texture on a grid of its own
-    for (int i = 0; i < num_cams; ++i) {  // canopies in camera order: the blend sums are order-dependent
-      CU(cudaMemcpy(s.disp.p, disparities[i], n * sizeof(float), cudaMemcpyDefault));
-      if (ps.color) CU(cudaMemcpy(s.bgra.p, colors_bgra[i], nc * 4 * sizeof(float), cudaMemcpyDefault));
-      CU(cudaMemset(s.flags.p, 0, sizeof(int)));
-      if (ownGrid) {
-        rephotoPrepKernel<<<dim3((cw + 127) / 128, ch), 128>>>(dcTex[i], nullptr, s.bgra.p, cw, ch, position[0], position[1],
-                                                              position[2], 0.0f, nullptr, texC, nullptr, s.flags.p);
-        rephotoPrepKernel<<<dim3((mw + 127) / 128, mh), 128>>>(dcMesh[i], s.disp.p, nullptr, mw, mh, position[0],
-                                                              position[1], position[2], ipd, s.vtx.p, nullptr, nullptr,
-                                                              s.flags.p);
-      } else {
-        rephotoPrepKernel<<<dim3((mw + 127) / 128, mh), 128>>>(dcMesh[i], s.disp.p, s.bgra.p, mw, mh, position[0],
-                                                              position[1], position[2], ipd, s.vtx.p, texC, texD,
-                                                              s.flags.p);
-      }
-      for (int l = 1; l < levels; ++l)
-        for (int t = 0; t < 2; ++t) {
-          ushort4* tex = t == 0 ? texC : texD;
-          if (!tex) continue;
-          rephotoMipKernel<<<dim3((cv.lw[l] + 127) / 128, cv.lh[l]), 128>>>(tex + cv.lofs[l - 1], cv.lw[l - 1],
-                                                                            cv.lh[l - 1], tex + cv.lofs[l], cv.lw[l],
-                                                                            cv.lh[l]);
-        }
-      CU(cudaMemcpy(&cv.anyZeroAlpha, s.flags.p, sizeof(int), cudaMemcpyDeviceToHost));
-      CU(cudaMemset(s.keys.p, 0xff, pixels * sizeof(unsigned long long)));
-      rephotoRasterKernel<<<dim3((prims + 255) / 256, views), 256>>>(cv, s.mats.p, W, H, prims, s.keys.p);
-      rephotoResolveKernel<<<grid1(pixels), 256>>>(cv, s.mats.p, W, H, views, s.keys.p, ps.color ? s.accC.p : nullptr,
-                                                   ps.disp ? s.accD.p : nullptr, win ? win + (size_t)i * pixels : nullptr);
-      CU(cudaGetLastError());
-    }
-  }
-  std::vector<float> trig;
-  if (projection == DERP_CANOPY_EQUIRECT) {  // equirectFS' texel-centre directions, fp64 rounded to fp32
-    const int e = outH;
-    trig.resize((size_t)6 * e);
-    const double kPi = 3.14159265358979323846;
-    for (int y = 0; y < e; ++y) {
-      const double lat = -(((y + 0.5) / e) - 0.5) * kPi;
-      trig[y] = (float)std::cos(lat);
-      trig[e + y] = (float)std::sin(lat);
-    }
-    for (int x = 0; x < 2 * e; ++x) {
-      const double lon = (1 - (x + 0.5) / (2 * e)) * 2.0 * kPi;
-      trig[2 * e + x] = (float)std::cos(lon);
-      trig[4 * e + x] = (float)std::sin(lon);
-    }
-    CU(s.trig.ensure(trig.size()));
-    CU(cudaMemcpy(s.trig.p, trig.data(), trig.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CU(s.eq.ensure((size_t)2 * e * e * 4));
-  }
-  for (int t = 0; t < 2; ++t) {
-    float* dst = t == 0 ? out_color : out_disparity;
-    if (!dst) continue;
-    rephotoUnpremulKernel<<<grid1(pixels), 256>>>(pixels, t == 0 ? s.accC.p : s.accD.p, zeroNan, s.out.p);
-    CU(cudaGetLastError());
-    if (projection == DERP_CANOPY_EQUIRECT) {
-      const int e = outH;
-      canopyEquirectKernel<<<dim3((2 * e + 127) / 128, e), 128>>>(s.out.p, e, s.trig.p, s.eq.p);
-      CU(cudaGetLastError());
-      CU(cudaMemcpy(dst, s.eq.p, (size_t)2 * e * e * 4 * sizeof(float), cudaMemcpyDefault));
-    } else {
-      CU(cudaMemcpy(dst, s.out.p, pixels * 4 * sizeof(float), cudaMemcpyDefault));
-    }
-  }
-  if (winners && num_cams > 0)
-    CU(cudaMemcpy(winners, s.win.p, pixels * num_cams * sizeof(int32_t), cudaMemcpyDefault));
-  CU(cudaDeviceSynchronize());
-  return DERP_OK;
-}
-}  // namespace
-
-extern "C" {
-
-int derp_rephoto_cubemap(int device, const DerpCameraDesc* cams, int num_cams, const float* const* disparities,
-                         const float* const* colors_bgra, int width, int height, const float* center, int edge,
-                         float* out_color, float* out_disparity, int32_t* winners) {
-  return canopyRender("derp_rephoto_cubemap", device, cams, num_cams, disparities, width, height, colors_bgra, width, height,
-                      DERP_CANOPY_CUBEMAP, center, nullptr, edge, edge, 0.0f, 1, DERP_CANOPY_ON_SCREEN, true, out_color,
-                      out_disparity, winners);
-}
-
-int derp_canopy_render(int device, const DerpCameraDesc* cams, int num_cams, const float* const* disparities,
-                       int mesh_width, int mesh_height, const float* const* colors_bgra, int color_width,
-                       int color_height, int projection, const float* position, const float* matrix, int out_width,
-                       int out_height, float ipd, int alpha_blend, int shader, float* out_color, float* out_disparity,
-                       int32_t* winners) {
-  return canopyRender("derp_canopy_render", device, cams, num_cams, disparities, mesh_width, mesh_height, colors_bgra,
-                      color_width, color_height, projection, position, matrix, out_width, out_height, ipd, alpha_blend,
-                      shader, false, out_color, out_disparity, winners);
-}
-
-int derp_canopy_snapshot_matrix(const float* position, const float* forward, const float* up, double horizontal_fov_deg,
-                                int width, int height, float* matrix) {
-  if (!position || !forward || !up || !matrix || width < 1 || height < 1)
-    return fail(DERP_EINVAL, "derp_canopy_snapshot_matrix: bad arguments");
-  if (!derp::rephoto::snapshotMatrix(position, forward, up, horizontal_fov_deg, width, height, matrix))
-    return fail(DERP_EINVAL, "derp_canopy_snapshot_matrix: forward and up do not give a unitary basis");
-  return DERP_OK;
-}
-
-int derp_rephoto_score(int device, const float* ref_bgr, const float* ren_bgr, const uint8_t* mask, int width, int height,
-                       int method, int stat_radius, float* score_map, double* avg) {
-  using namespace derp::rephoto;
-  if (!ref_bgr || !ren_bgr || !mask || width < 1 || height < 1 || !score_map || !avg)
-    return fail(DERP_EINVAL, "derp_rephoto_score: bad arguments");
-  if (method != DERP_REPHOTO_MSSIM && method != DERP_REPHOTO_NCC)
-    return fail(DERP_EINVAL, "derp_rephoto_score: method must be DERP_REPHOTO_MSSIM or DERP_REPHOTO_NCC");
-  if (stat_radius < 1 || stat_radius > 31) return fail(DERP_EINVAL, "derp_rephoto_score: stat_radius in [1, 31]");
-  int rc = rephotoScratch(device);
-  if (rc) return rc;
-  RephotoScratch& s = g_rephoto;
-  const size_t pixels = (size_t)width * height, n = pixels * 3;
-  // f32 layout: [x | y | mu (2n) | moments (3n) | sig (3n) | tmp (3n) | weights (64)]
-  CU(s.f32.ensure(13 * n + 64));
-  float *x = s.f32.p, *y = x + n, *mu = y + n, *mom = mu + 2 * n, *sig = mom + 3 * n, *tmp = sig + 3 * n,
-        *wt = tmp + 3 * n;
-  float hw[64];
-  gaussianWeights(stat_radius, hw);
-  const unsigned blocks = grid1(pixels);
-  CU(s.mask.ensure(pixels));
-  CU(s.out.ensure(n));
-  CU(s.partial.ensure((size_t)blocks * 6));
-  CU(cudaMemcpy(x, ref_bgr, n * sizeof(float), cudaMemcpyDefault));
-  CU(cudaMemcpy(y, ren_bgr, n * sizeof(float), cudaMemcpyDefault));
-  CU(cudaMemcpy(s.mask.p, mask, pixels, cudaMemcpyDefault));
-  CU(cudaMemcpy(wt, hw, (2 * stat_radius + 1) * sizeof(float), cudaMemcpyHostToDevice));
-  const dim3 g2((width + 127) / 128, height, 2), g3((width + 127) / 128, height, 3);
-  rephotoBlurRowsKernel<<<g2, 128>>>(x, width, height, stat_radius, wt, tmp);  // x, y are adjacent: two images
-  rephotoBlurColsKernel<<<g2, 128>>>(tmp, width, height, stat_radius, wt, mu);
-  rephotoMomentsKernel<<<grid1(n), 256>>>(n, x, y, mu, mom);
-  rephotoBlurRowsKernel<<<g3, 128>>>(mom, width, height, stat_radius, wt, tmp);
-  rephotoBlurColsKernel<<<g3, 128>>>(tmp, width, height, stat_radius, wt, sig);
-  rephotoScoreKernel<<<blocks, 256>>>(pixels, mu, sig, s.mask.p, method == DERP_REPHOTO_NCC, s.out.p, s.partial.p);
-  CU(cudaGetLastError());
-  std::vector<double> part((size_t)blocks * 6);
-  CU(cudaMemcpy(score_map, s.out.p, n * sizeof(float), cudaMemcpyDefault));
-  CU(cudaMemcpy(part.data(), s.partial.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  for (int c = 0; c < 3; ++c) {  // cv::mean(channel, mask without NaN): 0 for an empty mask
-    double sum = 0, cnt = 0;
-    for (unsigned b = 0; b < blocks; ++b) {
-      sum += part[b * 6 + c];
-      cnt += part[b * 6 + 3 + c];
-    }
-    avg[c] = cnt > 0 ? sum / cnt : 0.0;
-  }
-  return DERP_OK;
-}
-
 }  // extern "C"
 
 // ---- host-side test hooks ---------------------------------------------------------------------------
@@ -2382,37 +1727,6 @@ int derp_test_select_table(const float* first, const float* second, int n, int k
   return ok8 ? 1 : 0;
 }
 
-// host-only hook for tests/test_mesh.py: the simplifier on an arbitrary mesh (double xyz, uint32 indices); outputs sized
-// like the inputs
-int derp_test_simplify(const double* xyz, uint64_t nv, const uint32_t* idx, uint64_t nf, int triangles, float strictness,
-                       int remove_boundary_edges, double* out_xyz, uint32_t* out_idx, uint64_t* out_nv, uint64_t* out_nf) {
-  derp::simplify::Mesh mesh(xyz, nv, idx, nf);
-  mesh.run(triangles, strictness, remove_boundary_edges != 0);
-  for (size_t i = 0; i < mesh.verts.size(); ++i) {
-    out_xyz[3 * i] = mesh.verts[i].p.x;
-    out_xyz[3 * i + 1] = mesh.verts[i].p.y;
-    out_xyz[3 * i + 2] = mesh.verts[i].p.z;
-  }
-  for (size_t i = 0; i < mesh.faces.size(); ++i)
-    for (int j = 0; j < 3; ++j) out_idx[3 * i + j] = (uint32_t)mesh.faces[i].v[j];
-  *out_nv = mesh.verts.size();
-  *out_nf = mesh.faces.size();
-  return 0;
-}
-
-// HOST instantiation of the BC7 block encoder (derp_bc7.cuh) for tests/test_bc7.py -m "not gpu"; the apps call
-// derp_bc7_compress* (CUDA) only.
-int derp_test_bc7_blocks_host(const uint8_t* rgba, int width, int height, uint8_t* blocks) {
-  if (!rgba || !blocks || width < 1 || height < 1) return DERP_EINVAL;
-  std::memset(blocks, 0, (size_t)width * height);
-  derp::bc7::encodeSurfaceOnHost(rgba, width, height, blocks);
-  return DERP_OK;
-}
-int derp_test_bc7_gamma_table(int bits_per_channel, float gamma, uint8_t* lut) {
-  if ((bits_per_channel != 8 && bits_per_channel != 16) || !lut) return DERP_EINVAL;
-  derp::bc7::gammaTable(bits_per_channel, gamma, lut);
-  return DERP_OK;
-}
 
 float derp_test_robust_sum(const float* first, const float* second, int n, int keep) {
   float a[64], b[64];
@@ -2464,398 +1778,6 @@ int derp_test_camera_info(const DerpCameraDesc* d, double* rotation9, double* di
   for (int i = 0; i < 9; ++i) rotation9[i] = c.rot[i];
   *distortion_max = c.distMax;
   *cos_fov = c.cosFov;
-  return DERP_OK;
-}
-
-}  // extern "C"
-
-// ---- sweep-view slices (derp_sweepview.h) ---------------------------------------------------------------------
-namespace {
-using derp::sweep::SrcImage;
-
-struct SweepScratch {
-  DevBuf<DevCamera> cams;
-  DevBuf<SrcImage> imgs;
-  DevBuf<float4> upload, out;
-  DevBuf<double> tabs;
-  DevBuf<float> depths;
-  DevBuf<int> widths, box;
-  DevBuf<float4*> outs;
-  DevBuf<unsigned long long> hits;
-  int device = -1;
-  void release() {
-    cams.release(); imgs.release(); upload.release(); out.release(); tabs.release(); depths.release();
-    widths.release(); box.release(); outs.release(); hits.release();
-  }
-};
-thread_local SweepScratch g_sweep;
-thread_local unsigned long long g_sweepHits = 0;  // contributing (sample, camera) pairs of the last call
-
-int sweepScratch(int device) {
-  SweepScratch& s = g_sweep;
-  if (s.device != device) {
-    if (s.device >= 0) {
-      cudaSetDevice(s.device);
-      s.release();
-    }
-    s.device = device;
-  }
-  CU(cudaSetDevice(device));
-  return DERP_OK;
-}
-
-// Cameras as the apps hold them (already rescaled), optionally centred on camera `center`
-int sweepCameras(const char* who, const DerpCameraDesc* cams, int n, int center, std::vector<DevCamera>& out) {
-  const std::string name(who);
-  if (!cams || n < 1 || n > derp::sweep::kMaxCams)
-    return fail(DERP_EINVAL, name + ": between 1 and " + std::to_string(derp::sweep::kMaxCams) + " cameras");
-  std::vector<DerpCameraDesc> d(cams, cams + n);
-  if (center >= n) return fail(DERP_EINVAL, name + ": center index out of range");
-  if (center >= 0 && !derp::sweep::host::centerRig(d.data(), n, center))
-    return fail(DERP_EINVAL, name + ": centerRig produced an invalid rotation");
-  out.resize(n);
-  for (int i = 0; i < n; ++i)
-    if (!host::makeCamera(d[i], &out[i])) return fail(DERP_EINVAL, name + ": invalid camera " + std::to_string(i));
-  return DERP_OK;
-}
-
-int checkImages(const char* who, const float* const* images, const int32_t* sizes, int n) {
-  if (!images || !sizes) return fail(DERP_EINVAL, std::string(who) + ": images and sizes are required");
-  for (int i = 0; i < n; ++i)
-    if (!images[i] || sizes[2 * i] < 1 || sizes[2 * i + 1] < 1 || (long long)sizes[2 * i] * sizes[2 * i + 1] >= (1ll << 30))
-      return fail(DERP_EINVAL, std::string(who) + ": bad image " + std::to_string(i));
-  return DERP_OK;
-}
-
-// The equirect reads images[c](int(py), int(px)) unclamped: every camera's resolution must fit its image
-int checkFit(const char* who, const std::vector<DevCamera>& c, const int32_t* sizes) {
-  for (size_t i = 0; i < c.size(); ++i)
-    if (c[i].res[0] > sizes[2 * i] || c[i].res[1] > sizes[2 * i + 1])
-      return fail(DERP_EINVAL, std::string(who) + ": camera " + std::to_string(i) + "'s resolution " +
-                                   std::to_string(c[i].res[0]) + " x " + std::to_string(c[i].res[1]) +
-                                   " exceeds its image " + std::to_string(sizes[2 * i]) + " x " +
-                                   std::to_string(sizes[2 * i + 1]));
-  return DERP_OK;
-}
-
-// Device copies of the rig and its images: device-resident images are used in place (16-byte aligned float4)
-int stageSweepRig(const std::vector<DevCamera>& cams, const float* const* images, const int32_t* sizes) {
-  SweepScratch& s = g_sweep;
-  const int n = (int)cams.size();
-  CU(s.cams.ensure(n));
-  CU(cudaMemcpy(s.cams.p, cams.data(), n * sizeof(DevCamera), cudaMemcpyHostToDevice));
-  if (!images) return DERP_OK;
-  std::vector<SrcImage> im(n);
-  std::vector<size_t> hostAt(n, SIZE_MAX);
-  size_t total = 0;
-  for (int i = 0; i < n; ++i) {
-    cudaPointerAttributes at;
-    const bool dev = cudaPointerGetAttributes(&at, images[i]) == cudaSuccess && at.type == cudaMemoryTypeDevice &&
-                     ((uintptr_t)images[i] % 16) == 0;
-    cudaGetLastError();
-    if (!dev) {
-      hostAt[i] = total;
-      total += (size_t)sizes[2 * i] * sizes[2 * i + 1];
-    }
-    im[i] = SrcImage{reinterpret_cast<const float4*>(images[i]), sizes[2 * i], sizes[2 * i + 1]};
-  }
-  if (total) {
-    CU(s.upload.ensure(total));
-    for (int i = 0; i < n; ++i) {
-      if (hostAt[i] == SIZE_MAX) continue;
-      const size_t px = (size_t)sizes[2 * i] * sizes[2 * i + 1];
-      CU(cudaMemcpy(s.upload.p + hostAt[i], images[i], px * sizeof(float4), cudaMemcpyDefault));
-      im[i].p = s.upload.p + hostAt[i];
-    }
-  }
-  CU(s.imgs.ensure(n));
-  CU(cudaMemcpy(s.imgs.p, im.data(), n * sizeof(SrcImage), cudaMemcpyHostToDevice));
-  return DERP_OK;
-}
-
-size_t sweepSmem(int n) { return (size_t)n * (sizeof(DevCamera) + sizeof(SrcImage)); }
-
-// Host tables of one equirect slice set: full (bounds == NULL, one shared table) or cropped (one table per slice)
-struct EquirectPlan {
-  std::vector<double> cosT, sinT, sinP, cosP;
-  std::vector<int> widths;
-  int tStride = 0, pStride = 0, maxW = 0;
-};
-int planEquirect(const char* who, uint64_t height, int num, const double* bounds, EquirectPlan& p) {
-  if (height < 1 || height > (1u << 15)) return fail(DERP_EINVAL, std::string(who) + ": height must be 1..32768");
-  const double width = (double)(2 * height);
-  if (!bounds) {
-    std::vector<double> xs(2 * height), ys(height);
-    for (uint64_t i = 0; i < 2 * height; ++i) xs[i] = (double)i;
-    for (uint64_t i = 0; i < height; ++i) ys[i] = (double)i;
-    p.cosT.resize(xs.size()); p.sinT.resize(xs.size()); p.sinP.resize(height); p.cosP.resize(height);
-    derp::sweep::host::thetaTable(xs.data(), (int)xs.size(), width, p.cosT.data(), p.sinT.data());
-    derp::sweep::host::phiTable(ys.data(), (int)height, (double)height, p.sinP.data(), p.cosP.data());
-    p.widths.assign(num, (int)(2 * height));
-    p.maxW = (int)(2 * height);
-    return DERP_OK;
-  }
-  std::vector<uint64_t> ws(num);
-  for (int k = 0; k < num; ++k) {
-    if (!derp::sweep::host::cropWidth(height, bounds + 4 * k, &ws[k]))
-      return fail(DERP_EINVAL, std::string(who) + ": slice " + std::to_string(k) +
-                                   ": the crop box is empty or has zero width or height (nothing visible)");
-    p.maxW = std::max<int>(p.maxW, (int)ws[k]);
-  }
-  p.tStride = p.maxW;
-  p.pStride = (int)height;
-  p.cosT.assign((size_t)num * p.maxW, 0); p.sinT.assign((size_t)num * p.maxW, 0);
-  p.sinP.assign((size_t)num * height, 0); p.cosP.assign((size_t)num * height, 0);
-  for (int k = 0; k < num; ++k) {
-    std::vector<double> xs, ys;
-    derp::sweep::host::cropSamples(height, ws[k], bounds + 4 * k, xs, ys);
-    derp::sweep::host::thetaTable(xs.data(), (int)ws[k], width, &p.cosT[(size_t)k * p.maxW], &p.sinT[(size_t)k * p.maxW]);
-    derp::sweep::host::phiTable(ys.data(), (int)height, (double)height, &p.sinP[(size_t)k * height],
-                                &p.cosP[(size_t)k * height]);
-    p.widths.push_back((int)ws[k]);
-  }
-  return DERP_OK;
-}
-
-// Device copy of an EquirectPlan; `outs` (device pointers) are filled by the caller
-int uploadPlan(const EquirectPlan& p, const float* depths, int num, derp::sweep::EquirectSlices& s) {
-  SweepScratch& g = g_sweep;
-  const size_t nt = p.cosT.size(), np = p.sinP.size();
-  CU(g.tabs.ensure(2 * nt + 2 * np));
-  CU(cudaMemcpy(g.tabs.p, p.cosT.data(), nt * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(g.tabs.p + nt, p.sinT.data(), nt * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(g.tabs.p + 2 * nt, p.sinP.data(), np * 8, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(g.tabs.p + 2 * nt + np, p.cosP.data(), np * 8, cudaMemcpyHostToDevice));
-  CU(g.depths.ensure(num));
-  CU(cudaMemcpy(g.depths.p, depths, num * sizeof(float), cudaMemcpyDefault));
-  CU(g.widths.ensure(num));
-  CU(cudaMemcpy(g.widths.p, p.widths.data(), num * sizeof(int), cudaMemcpyHostToDevice));
-  s.cosT = g.tabs.p;
-  s.sinT = g.tabs.p + nt;
-  s.sinP = g.tabs.p + 2 * nt;
-  s.cosP = g.tabs.p + 2 * nt + np;
-  s.depths = g.depths.p;
-  s.widths = g.widths.p;
-  s.tStride = p.tStride;
-  s.pStride = p.pStride;
-  s.height = (int)(p.sinP.size() / (p.pStride ? (size_t)num : 1));
-  s.numSlices = num;
-  return DERP_OK;
-}
-
-// an output the kernels can write in place: device memory, 16-byte aligned for float4 stores.  Anything else is staged
-// in scratch and copied back with cudaMemcpyDefault, which infers the direction from the address
-bool onDevice(const void* p) {
-  cudaPointerAttributes at;
-  const bool d = cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeDevice &&
-                 ((uintptr_t)p % 16) == 0;
-  cudaGetLastError();
-  return d;
-}
-
-}  // namespace
-
-extern "C" {
-
-int derp_sweep_overlaps(int device, const DerpCameraDesc* cams, int num_cams, const float* const* images_bgra,
-                        const int32_t* image_sizes, int dst, const float* disparities, int num_slices, float* out) {
-  static const char* who = "derp_sweep_overlaps";
-  std::vector<DevCamera> c;
-  if (int rc = sweepCameras(who, cams, num_cams, -1, c)) return rc;
-  if (int rc = checkImages(who, images_bgra, image_sizes, num_cams)) return rc;
-  if (dst < 0 || dst >= num_cams || !disparities || num_slices < 1 || !out)
-    return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
-  const int W = (int)c[dst].res[0], H = (int)c[dst].res[1];  // Image colorDst(resolution.y(), resolution.x())
-  if (W < 1 || H < 1) return fail(DERP_EINVAL, std::string(who) + ": the destination has no pixels");
-  if ((long long)W * H * num_slices >= (1ll << 31)) return fail(DERP_EINVAL, std::string(who) + ": output too large");
-  if (int rc = sweepScratch(device)) return rc;
-  if (int rc = stageSweepRig(c, images_bgra, image_sizes)) return rc;
-  SweepScratch& s = g_sweep;
-  const size_t plane = (size_t)W * H;
-  float4* dOut;
-  if (onDevice(out)) {
-    dOut = reinterpret_cast<float4*>(out);
-  } else {
-    CU(s.out.ensure(plane * num_slices));
-    dOut = s.out.p;
-  }
-  CU(s.depths.ensure(num_slices));
-  CU(cudaMemcpy(s.depths.p, disparities, num_slices * sizeof(float), cudaMemcpyDefault));
-  CU(s.hits.ensure(1));
-  CU(cudaMemset(s.hits.p, 0, sizeof(unsigned long long)));
-  const int chunk = derp::sweep::kOverlapSlicesPerThread;
-  const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
-  const dim3 grid((W + block.x - 1) / block.x, (H + block.y - 1) / block.y, (num_slices + chunk - 1) / chunk);
-  derp::sweep::overlapsKernel<<<grid, block, sweepSmem(num_cams)>>>(s.cams.p, s.imgs.p, num_cams, dst, W, H, s.depths.p,
-                                                                     num_slices, chunk, dOut, s.hits.p);
-  CU(cudaGetLastError());
-  if (dOut != reinterpret_cast<float4*>(out))
-    CU(cudaMemcpy(out, dOut, plane * num_slices * sizeof(float4), cudaMemcpyDefault));
-  CU(cudaMemcpy(&g_sweepHits, s.hits.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  return DERP_OK;
-}
-
-int derp_sweep_crop_bounds(int device, const DerpCameraDesc* cams, int num_cams, int center, uint64_t height,
-                           const float* depths, int num_depths, double* bounds) {
-  static const char* who = "derp_sweep_crop_bounds";
-  std::vector<DevCamera> c;
-  if (int rc = sweepCameras(who, cams, num_cams, center, c)) return rc;
-  if (!depths || num_depths < 1 || num_depths > 65535 || !bounds)
-    return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
-  EquirectPlan p;
-  if (int rc = planEquirect(who, height, num_depths, nullptr, p)) return rc;
-  if (int rc = sweepScratch(device)) return rc;
-  if (int rc = stageSweepRig(c, nullptr, nullptr)) return rc;
-  derp::sweep::EquirectSlices sl{};
-  if (int rc = uploadPlan(p, depths, num_depths, sl)) return rc;
-  SweepScratch& s = g_sweep;
-  std::vector<int> box(4 * num_depths);
-  for (int k = 0; k < num_depths; ++k) {
-    box[4 * k] = (int)(2 * height);  // minX = width, maxX = 0, minY = height, maxY = 0
-    box[4 * k + 1] = 0;
-    box[4 * k + 2] = (int)height;
-    box[4 * k + 3] = 0;
-  }
-  CU(s.box.ensure(box.size()));
-  CU(cudaMemcpy(s.box.p, box.data(), box.size() * sizeof(int), cudaMemcpyHostToDevice));
-  const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
-  const dim3 grid((p.maxW + block.x - 1) / block.x, ((int)height + block.y - 1) / block.y, num_depths);
-  derp::sweep::cropBoundsKernel<<<grid, block, sweepSmem(num_cams)>>>(s.cams.p, num_cams, sl, s.box.p);
-  CU(cudaGetLastError());
-  CU(cudaMemcpy(box.data(), s.box.p, box.size() * sizeof(int), cudaMemcpyDeviceToHost));
-  for (size_t i = 0; i < box.size(); ++i) bounds[i] = (double)box[i];
-  return DERP_OK;
-}
-
-int derp_sweep_crop_width(uint64_t height, const double* bounds, uint64_t* width) {
-  if (!bounds || !width) return fail(DERP_EINVAL, "derp_sweep_crop_width: bad arguments");
-  if (!derp::sweep::host::cropWidth(height, bounds, width))
-    return fail(DERP_EINVAL, "derp_sweep_crop_width: the crop box is empty or has zero width or height (nothing visible)");
-  return DERP_OK;
-}
-
-int derp_sweep_equirect(int device, const DerpCameraDesc* cams, int num_cams, int center, const float* const* images_bgra,
-                        const int32_t* image_sizes, uint64_t height, const float* depths, int num_depths,
-                        const double* bounds, int black_bg, float* const* out) {
-  static const char* who = "derp_sweep_equirect";
-  std::vector<DevCamera> c;
-  if (int rc = sweepCameras(who, cams, num_cams, center, c)) return rc;
-  if (int rc = checkImages(who, images_bgra, image_sizes, num_cams)) return rc;
-  if (int rc = checkFit(who, c, image_sizes)) return rc;
-  if (!depths || num_depths < 1 || num_depths > 65535 || !out) return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
-  for (int k = 0; k < num_depths; ++k)
-    if (!out[k]) return fail(DERP_EINVAL, std::string(who) + ": NULL output");
-  EquirectPlan p;
-  if (int rc = planEquirect(who, height, num_depths, bounds, p)) return rc;
-  if (int rc = sweepScratch(device)) return rc;
-  if (int rc = stageSweepRig(c, images_bgra, image_sizes)) return rc;
-  derp::sweep::EquirectSlices sl{};
-  if (int rc = uploadPlan(p, depths, num_depths, sl)) return rc;
-  SweepScratch& s = g_sweep;
-  // device-resident outputs are written in place; the others are staged in one scratch buffer and copied back
-  std::vector<float4*> outs(num_depths);
-  std::vector<size_t> at(num_depths, SIZE_MAX);
-  size_t total = 0;
-  for (int k = 0; k < num_depths; ++k) {
-    if (onDevice(out[k])) continue;
-    at[k] = total;
-    total += (size_t)p.widths[k] * height;
-  }
-  if (total) CU(s.out.ensure(total));
-  for (int k = 0; k < num_depths; ++k)
-    outs[k] = at[k] == SIZE_MAX ? reinterpret_cast<float4*>(out[k]) : s.out.p + at[k];
-  CU(s.outs.ensure(num_depths));
-  CU(cudaMemcpy(s.outs.p, outs.data(), num_depths * sizeof(float4*), cudaMemcpyHostToDevice));
-  sl.outs = s.outs.p;
-  CU(s.hits.ensure(1));
-  CU(cudaMemset(s.hits.p, 0, sizeof(unsigned long long)));
-  const float4 bg = black_bg ? make_float4(0.f, 0.f, 0.f, 1.f) : make_float4(0.f, 0.f, 1.f, 1.f);
-  const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
-  const dim3 grid((p.maxW + block.x - 1) / block.x, ((int)height + block.y - 1) / block.y, num_depths);
-  derp::sweep::equirectKernel<<<grid, block, sweepSmem(num_cams)>>>(s.cams.p, s.imgs.p, num_cams, sl, bg, s.hits.p);
-  CU(cudaGetLastError());
-  for (int k = 0; k < num_depths; ++k)
-    if (outs[k] != reinterpret_cast<float4*>(out[k]))
-      CU(cudaMemcpy(out[k], outs[k], (size_t)p.widths[k] * height * sizeof(float4), cudaMemcpyDefault));
-  CU(cudaMemcpy(&g_sweepHits, s.hits.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  return DERP_OK;
-}
-
-int derp_sweep_center_rig(const DerpCameraDesc* cams, int num_cams, int center, DerpCameraDesc* out, double* rotation9) {
-  if (!cams || num_cams < 1 || center < 0 || center >= num_cams || !out)
-    return fail(DERP_EINVAL, "derp_sweep_center_rig: bad arguments");
-  std::vector<DerpCameraDesc> d(cams, cams + num_cams);
-  if (!derp::sweep::host::centerRig(d.data(), num_cams, center))
-    return fail(DERP_EINVAL, "derp_sweep_center_rig: invalid camera rotation");
-  for (int i = 0; i < num_cams; ++i) {
-    out[i] = d[i];
-    if (rotation9) {
-      DevCamera c;
-      if (!host::makeCamera(d[i], &c)) return fail(DERP_EINVAL, "derp_sweep_center_rig: invalid camera");
-      for (int k = 0; k < 9; ++k) rotation9[9 * i + k] = c.rot[k];
-    }
-  }
-  return DERP_OK;
-}
-
-uint64_t derp_sweep_last_hits(void) { return g_sweepHits; }
-
-int derp_test_sweep_overlaps_host(const DerpCameraDesc* cams, int num_cams, const float* const* images_bgra,
-                                  const int32_t* image_sizes, int dst, const float* disparities, int num_slices,
-                                  float* out) {
-  static const char* who = "derp_test_sweep_overlaps_host";
-  std::vector<DevCamera> c;
-  if (int rc = sweepCameras(who, cams, num_cams, -1, c)) return rc;
-  if (int rc = checkImages(who, images_bgra, image_sizes, num_cams)) return rc;
-  if (dst < 0 || dst >= num_cams || !disparities || num_slices < 1 || !out) return fail(DERP_EINVAL, "bad arguments");
-  std::vector<SrcImage> im(num_cams);
-  for (int i = 0; i < num_cams; ++i)
-    im[i] = SrcImage{reinterpret_cast<const float4*>(images_bgra[i]), image_sizes[2 * i], image_sizes[2 * i + 1]};
-  const int W = (int)c[dst].res[0], H = (int)c[dst].res[1];
-  float4* o = reinterpret_cast<float4*>(out);
-  int hits = 0;
-  for (int y = 0; y < H; ++y)
-    for (int x = 0; x < W; ++x) {
-      const double px = x + 0.5, py = y + 0.5;
-      const bool outside = outsideImageCircle(c[dst], px, py);
-      double dir[3];
-      if (!outside) pixelRay(c[dst], px, py, dir);
-      for (int k = 0; k < num_slices; ++k)
-        o[(size_t)k * W * H + (size_t)y * W + x] =
-            outside ? make_float4(0.f, 0.f, 0.f, 0.f)
-                    : derp::sweep::overlapPixel(c.data(), im.data(), num_cams, c[dst].pos, dir, disparities[k], &hits);
-    }
-  return DERP_OK;
-}
-
-int derp_test_sweep_equirect_host(const DerpCameraDesc* cams, int num_cams, int center,
-                                  const float* const* images_bgra, const int32_t* image_sizes, uint64_t height,
-                                  const float* depths, int num_depths, const double* bounds, int black_bg,
-                                  float* const* out) {
-  static const char* who = "derp_test_sweep_equirect_host";
-  std::vector<DevCamera> c;
-  if (int rc = sweepCameras(who, cams, num_cams, center, c)) return rc;
-  if (int rc = checkImages(who, images_bgra, image_sizes, num_cams)) return rc;
-  if (int rc = checkFit(who, c, image_sizes)) return rc;
-  if (!depths || num_depths < 1 || !out) return fail(DERP_EINVAL, "bad arguments");
-  EquirectPlan p;
-  if (int rc = planEquirect(who, height, num_depths, bounds, p)) return rc;
-  std::vector<SrcImage> im(num_cams);
-  for (int i = 0; i < num_cams; ++i)
-    im[i] = SrcImage{reinterpret_cast<const float4*>(images_bgra[i]), image_sizes[2 * i], image_sizes[2 * i + 1]};
-  const float4 bg = black_bg ? make_float4(0.f, 0.f, 0.f, 1.f) : make_float4(0.f, 0.f, 1.f, 1.f);
-  int hits = 0;
-  for (int k = 0; k < num_depths; ++k) {
-    const double depth = (double)depths[k];
-    const int W = p.widths[k];
-    for (uint64_t y = 0; y < height; ++y)
-      for (int x = 0; x < W; ++x) {
-        const double r = depth * p.sinP[(size_t)k * p.pStride + y];
-        reinterpret_cast<float4*>(out[k])[y * W + x] = derp::sweep::equirectPixel(
-            c.data(), im.data(), num_cams, r * p.cosT[(size_t)k * p.tStride + x], r * p.sinT[(size_t)k * p.tStride + x],
-            depth * p.cosP[(size_t)k * p.pStride + y], bg, &hits);
-      }
-  }
   return DERP_OK;
 }
 

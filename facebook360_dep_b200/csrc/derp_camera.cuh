@@ -282,7 +282,7 @@ DERP_HD double undistort(const DevCamera& c, double y) {  // Camera.h:243-284
 // (visible in the SASS); this one issues ~45 instructions in total.  Error < 1.5 ulp, i.e. the same
 // tolerance class as CUDA-vs-glibc atan2 (the value is narrowed to fp32 pixel coordinates afterwards).
 #if defined(__CUDACC__)
-__constant__ double kAtanT[11] = {
+static __constant__ double kAtanT[11] = {  // static: one copy per translation unit that includes this header
     3.33333333333329318027e-01,  -1.99999999998764832476e-01, 1.42857142725034663711e-01,
     -1.11111104054623557880e-01, 9.09088713343650656196e-02,  -7.69187620504482999495e-02,
     6.66107313738753120669e-02,  -5.83357013379057348645e-02, 4.97687799461593236017e-02,
