@@ -828,3 +828,48 @@ class SweepView(_Binding):
         self._check(self.lib.derp_sweep_center_rig(descs, len(descs), center, out, rot.ctypes.data))
         org = np.array([[out[i].origin[k] for k in range(3)] for i in range(len(descs))], np.float64)
         return out, rot, org
+
+
+# ---- include/derp_eqrmesh.h ---------------------------------------------------------------------------------------
+_EQR_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_equirect_mesh_size": (C.c_int, [C.c_int, C.c_int, C.c_double, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "derp_equirect_mesh": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_float, C.c_void_p,
+                                     C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "derp_equirect_mesh_simplified": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_float,
+                                                C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64),
+                                                C.POINTER(C.c_uint64)]),
+}
+EQR_SYMBOLS = sorted(k for k in _EQR_SIGS if k.startswith("derp_equirect_"))
+
+
+class EqrMesh(_Binding):
+    """ctypes binding of include/derp_eqrmesh.h on a loaded library: ``EqrMesh(load_cuda())`` for the product, or a path
+    to a library exporting the same entry points (the CPU checkers the tests build)."""
+
+    def __init__(self, library):
+        self.path, self.lib = _bind(library, _EQR_SIGS)
+
+    def mesh(self, disparity, scale=1.0, max_depth=700.0, tear_ratio=0.95, num_faces=200000, strictness=0.0,
+             device=0):
+        """CreateObjFromDisparityEquirect's mesh of a disparity equirect (float32 [h, w], or a device pointer given as
+        (ptr, w, h)): returns (vertexes float64 [nv, 3], faces uint32 [nf, 3]); simplified when strictness > 0."""
+        if isinstance(disparity, tuple):
+            ptr, w, h = disparity
+        else:
+            disparity = np.ascontiguousarray(disparity, np.float32)
+            h, w = disparity.shape
+            ptr = disparity.ctypes.data
+        mw, mh = C.c_int(), C.c_int()
+        self._check(self.lib.derp_equirect_mesh_size(w, h, scale, C.byref(mw), C.byref(mh)))
+        cells = mw.value * mh.value
+        vtx = np.empty((cells, 3), np.float64)
+        idx = np.empty((2 * cells, 3), np.uint32)
+        nv, nf = C.c_uint64(), C.c_uint64()
+        head = (device, ptr, w, h, float(scale), float(max_depth), tear_ratio)
+        tail = (vtx.ctypes.data, idx.ctypes.data, C.byref(nv), C.byref(nf))
+        if strictness > 0:
+            self._check(self.lib.derp_equirect_mesh_simplified(*head, int(num_faces), float(strictness), *tail))
+        else:
+            self._check(self.lib.derp_equirect_mesh(*head, *tail))
+        return vtx[:nv.value].copy(), idx[:nf.value].copy()

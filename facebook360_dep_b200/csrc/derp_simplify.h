@@ -98,16 +98,23 @@ class Mesh {
   std::vector<uint32_t> failed;   // per edge (3 per face): 1 + number of contractions done when it last failed, 0 = not known
   std::vector<uint32_t> stamped;  // per vertex: number of the last contraction that touched its closed 1-ring
   uint32_t contractions = 0;
+  // MeshSimplifier's isEquiError: false divides every cost by the squared norm of the contraction target
+  // (MeshSimplifier.cpp:165-169), for meshes in rig coordinates, where the same error matters less further away
+  bool equiError = true;
 
   // xyz: 3 doubles per vertex; idx: 3 indices per face
-  Mesh(const double* xyz, size_t nv, const uint32_t* idx, size_t nf) : verts(nv), faces(nf), cost(3 * nf), flag(nf, 0), admissible(3 * nf, 1), failed(3 * nf, 0), stamped(nv, 0) {
+  Mesh(const double* xyz, size_t nv, const uint32_t* idx, size_t nf, bool isEquiError = true) : verts(nv), faces(nf), cost(3 * nf), flag(nf, 0), admissible(3 * nf, 1), failed(3 * nf, 0), stamped(nv, 0), equiError(isEquiError) {
     for (size_t i = 0; i < nv; ++i) verts[i].p = V3{xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]};
     for (size_t i = 0; i < nf; ++i)
       for (int j = 0; j < 3; ++j) faces[i].v[j] = (int)idx[3 * i + j];
   }
 
-  // optimal position of the vertex an edge contracts to, and the error there (computeError, equi-error variant)
+  // optimal position of the vertex an edge contracts to, and the cost of contracting there (computeError)
   double contraction(const Vertex& a, const Vertex& b, V3* target) const {
+    const double e = quadricContraction(a, b, target);
+    return equiError ? e : e / dot(*target, *target);
+  }
+  double quadricContraction(const Vertex& a, const Vertex& b, V3* target) const {
     Quadric q = a.q;
     addInto(q, b.q);
     double top[3][3];
