@@ -90,8 +90,7 @@ int canopyRender(const char* who, int device, const DerpCameraDesc* cams, int nu
   CU(s.vtx.ensure(n * 3));
   CU(s.keys.ensure(pixels));
   CU(s.flags.ensure(1));
-  CU(s.mats.ensure(mats.size()));
-  CU(cudaMemcpy(s.mats.p, mats.data(), mats.size() * sizeof(float), cudaMemcpyHostToDevice));
+  if (int rc = upload(s.mats, mats.data(), mats.size())) return rc;
   if (out_color) {
     CU(s.bgra.ensure(nc * 4));
     CU(s.accC.ensure(pixels));
@@ -178,8 +177,7 @@ int canopyRender(const char* who, int device, const DerpCameraDesc* cams, int nu
       trig[2 * e + x] = (float)std::cos(lon);
       trig[4 * e + x] = (float)std::sin(lon);
     }
-    CU(s.trig.ensure(trig.size()));
-    CU(cudaMemcpy(s.trig.p, trig.data(), trig.size() * sizeof(float), cudaMemcpyHostToDevice));
+    if (int rc = upload(s.trig, trig.data(), trig.size())) return rc;
     CU(s.eq.ensure((size_t)2 * e * e * 4));
   }
   for (int t = 0; t < 2; ++t) {

@@ -80,8 +80,7 @@ static int cameraMesh(int device, const float* disparity, int width, int height,
   if ((rc = stageIn(disp, nsrc, dDisp))) return rc;
   if (fg && (rc = stageIn(fg, (size_t)mask_width * mask_height, dFg))) return rc;
   const int tiles = (int)((n + kScanTile - 1) / kScanTile);
-  CU(dOfs.ensure(ofs.size()));
-  CU(cudaMemcpy(dOfs.p, ofs.data(), ofs.size() * sizeof(int), cudaMemcpyHostToDevice));
+  if ((rc = upload(dOfs, ofs.data(), ofs.size()))) return rc;
   CU(dQuad.ensure(n));
   CU(dUsed.ensure(n));
   CU(dTiles.ensure(2 * (size_t)tiles));
@@ -260,13 +259,10 @@ static int equirectMesh(int device, const float* disparity, int width, int heigh
     linearAxis(height, H, scale, false, yo, unused, yw);
     xo.insert(xo.end(), yo.begin(), yo.end());
     xw.insert(xw.end(), yw.begin(), yw.end());
-    CU(sc.dOfs.ensure(xo.size()));
-    CU(sc.dCopy.ensure(xc.size()));
-    CU(sc.dTables.ensure(xw.size()));
+    if ((rc = upload(sc.dOfs, xo.data(), xo.size())) || (rc = upload(sc.dCopy, xc.data(), xc.size())) ||
+        (rc = upload(sc.dTables, xw.data(), xw.size())))
+      return rc;
     CU(sc.dSmall.ensure(n));
-    CU(cudaMemcpy(sc.dOfs.p, xo.data(), xo.size() * sizeof(int), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(sc.dCopy.p, xc.data(), xc.size(), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(sc.dTables.p, xw.data(), xw.size() * sizeof(float), cudaMemcpyHostToDevice));
     const LinearTaps t{sc.dOfs.p, sc.dCopy.p, sc.dTables.p, sc.dOfs.p + W, sc.dTables.p + 2 * (size_t)W};
     resizeLinearKernel<<<grid2(W, H), block2()>>>(disp, width, t, W, H, sc.dSmall.p);
     CU(cudaGetLastError());
@@ -284,8 +280,7 @@ static int equirectMesh(int device, const float* disparity, int width, int heigh
     return rc;
   }
   DevBuf<float>& dAngles = sc.dAngles;
-  CU(dAngles.ensure(angles.size()));
-  CU(cudaMemcpy(dAngles.p, angles.data(), angles.size() * sizeof(float), cudaMemcpyHostToDevice));
+  if ((rc = upload(dAngles, angles.data(), angles.size()))) return rc;
   eqrVertexKernel<<<grid2(W, H), block2()>>>(W, H, disp, (float)max_depth, dAngles.p, dAngles.p + W,
                                              dAngles.p + 2 * W, dAngles.p + 2 * W + H, vtx);
   const int tiles = (int)((n + kScanTile - 1) / kScanTile);
@@ -359,12 +354,15 @@ static int bc7Launch(int device, const void* src, size_t srcBytes, int mode, int
                      const uint8_t* lutHost, size_t lutBytes, uint8_t* blocks) {
   CU(cudaSetDevice(device));
   const size_t outBytes = (size_t)width * height;
-  DevBuf<uint8_t> dSrc, dOut, dLut;
+  // grow-only scratch per host thread (the app converts one (frame, camera) after the other on each GPU worker thread)
+  static thread_local struct {
+    DevBuf<uint8_t> dSrc, dOut, dLut;
+  } sc;
   // 16-byte alignment: the RGBA source is read and the blocks are written as uint4
   const uint8_t* s = static_cast<const uint8_t*>(src);
   uint8_t* o = blocks;
-  int rc = stageIn(s, srcBytes, dSrc, 16);
-  if (rc || (rc = outBuffer(o, outBytes, dOut, 16))) return rc;
+  int rc = stageIn(s, srcBytes, sc.dSrc, 16);
+  if (rc || (rc = outBuffer(o, outBytes, sc.dOut, 16))) return rc;
   CU(cudaMemset(o, 0, outBytes));  // the reference's output vector starts zeroed; partial edge blocks are never written
   const int bx = width / 4, by = height / 4;
   if (bx > 0 && by > 0) {
@@ -372,19 +370,18 @@ static int bc7Launch(int device, const void* src, size_t srcBytes, int mode, int
     if (mode == 0) {
       derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(derp::bc7::Rgba8Source{(const uint8_t*)s, width}, width, bx, by, o);
     } else {
-      CU(dLut.ensure(lutBytes));
-      CU(cudaMemcpy(dLut.p, lutHost, lutBytes, cudaMemcpyHostToDevice));
+      if ((rc = upload(sc.dLut, lutHost, lutBytes))) return rc;
       if (mode == 8)
         derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(
-            derp::bc7::BgrSource<uint8_t>{(const uint8_t*)s, width, channels, dLut.p}, width, bx, by, o);
+            derp::bc7::BgrSource<uint8_t>{(const uint8_t*)s, width, channels, sc.dLut.p}, width, bx, by, o);
       else
         derp::bc7::bc7Kernel<<<grid, derp::bc7::kBc7Threads>>>(
-            derp::bc7::BgrSource<uint16_t>{(const uint16_t*)s, width, channels, dLut.p}, width, bx, by, o);
+            derp::bc7::BgrSource<uint16_t>{(const uint16_t*)s, width, channels, sc.dLut.p}, width, bx, by, o);
     }
     CU(cudaGetLastError());
   }
-  if (o != blocks) return stageOut(blocks, o, outBytes);
-  CU(cudaDeviceSynchronize());
+  if ((rc = stageOut(blocks, o, outBytes))) return rc;
+  CU(cudaDeviceSynchronize());  // return with blocks written, also when a staged copy goes to another GPU
   return DERP_OK;
 }
 

@@ -79,6 +79,21 @@ inline void nearestAxis(int sn, int dn, std::vector<int>& ofs) {
   for (int d = 0; d < dn; ++d) ofs[d] = std::min(floorD(d * ifx), sn - 1);
 }
 
+// Copies count elements of a host array the library built (a table, a camera) into buf, grown as needed
+template <typename T>
+int upload(DevBuf<T>& buf, const T* host, size_t count) {
+  CU(buf.ensure(count));
+  CU(cudaMemcpy(buf.p, host, count * sizeof(T), cudaMemcpyHostToDevice));
+  return DERP_OK;
+}
+// The same, stream-ordered on st
+template <typename T>
+int upload(DevBuf<T>& buf, const T* host, size_t count, cudaStream_t st) {
+  CU(buf.ensure(count));
+  CU(cudaMemcpyAsync(buf.p, host, count * sizeof(T), cudaMemcpyHostToDevice, st));
+  return DERP_OK;
+}
+
 // ---- caller pointers ----------------------------------------------------------------------------------------------
 // The device whose memory p is, or -1 for host, managed and unknown pointers
 inline int deviceOf(const void* p) {

@@ -60,8 +60,7 @@ int checkFit(const char* who, const std::vector<DevCamera>& c, const int32_t* si
 int stageSweepRig(const std::vector<DevCamera>& cams, const float* const* images, const int32_t* sizes) {
   SweepScratch& s = g_sweep;
   const int n = (int)cams.size();
-  CU(s.cams.ensure(n));
-  CU(cudaMemcpy(s.cams.p, cams.data(), n * sizeof(DevCamera), cudaMemcpyHostToDevice));
+  if (int rc = upload(s.cams, cams.data(), n)) return rc;
   if (!images) return DERP_OK;
   std::vector<SrcImage> im(n);
   std::vector<size_t> hostAt(n, SIZE_MAX);
@@ -82,9 +81,7 @@ int stageSweepRig(const std::vector<DevCamera>& cams, const float* const* images
       im[i].p = s.upload.p + hostAt[i];
     }
   }
-  CU(s.imgs.ensure(n));
-  CU(cudaMemcpy(s.imgs.p, im.data(), n * sizeof(SrcImage), cudaMemcpyHostToDevice));
-  return DERP_OK;
+  return upload(s.imgs, im.data(), n);
 }
 
 size_t sweepSmem(int n) { return (size_t)n * (sizeof(DevCamera) + sizeof(SrcImage)); }
@@ -142,8 +139,7 @@ int uploadPlan(const EquirectPlan& p, const float* depths, int num, derp::sweep:
   CU(cudaMemcpy(g.tabs.p + 2 * nt + np, p.cosP.data(), np * 8, cudaMemcpyHostToDevice));
   CU(g.depths.ensure(num));
   CU(cudaMemcpy(g.depths.p, depths, num * sizeof(float), cudaMemcpyDefault));
-  CU(g.widths.ensure(num));
-  CU(cudaMemcpy(g.widths.p, p.widths.data(), num * sizeof(int), cudaMemcpyHostToDevice));
+  if (int rc = upload(g.widths, p.widths.data(), num)) return rc;
   s.cosT = g.tabs.p;
   s.sinT = g.tabs.p + nt;
   s.sinP = g.tabs.p + 2 * nt;
@@ -214,8 +210,7 @@ int derp_sweep_crop_bounds(int device, const DerpCameraDesc* cams, int num_cams,
     box[4 * k + 2] = (int)height;
     box[4 * k + 3] = 0;
   }
-  CU(s.box.ensure(box.size()));
-  CU(cudaMemcpy(s.box.p, box.data(), box.size() * sizeof(int), cudaMemcpyHostToDevice));
+  if (int rc = upload(s.box, box.data(), box.size())) return rc;
   const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
   const dim3 grid((p.maxW + block.x - 1) / block.x, ((int)height + block.y - 1) / block.y, num_depths);
   derp::sweep::cropBoundsKernel<<<grid, block, sweepSmem(num_cams)>>>(s.cams.p, num_cams, sl, s.box.p);
@@ -262,8 +257,7 @@ int derp_sweep_equirect(int device, const DerpCameraDesc* cams, int num_cams, in
   if (total) CU(s.out.ensure(total));
   for (int k = 0; k < num_depths; ++k)
     outs[k] = at[k] == SIZE_MAX ? reinterpret_cast<float4*>(out[k]) : s.out.p + at[k];
-  CU(s.outs.ensure(num_depths));
-  CU(cudaMemcpy(s.outs.p, outs.data(), num_depths * sizeof(float4*), cudaMemcpyHostToDevice));
+  if (int rc = upload(s.outs, outs.data(), num_depths)) return rc;
   sl.outs = s.outs.p;
   CU(s.hits.ensure(1));
   CU(cudaMemset(s.hits.p, 0, sizeof(unsigned long long)));

@@ -11,7 +11,10 @@
  * Conventions
  *   - all functions return 0 on success, a negative DERP_E* code on failure;
  *     derp_last_error() returns a thread-local human readable message.
- *   - the caller owns every host pointer; the library owns device memory inside DerpCtx.
+ *   - in the CUDA library, every image, plane, mask and output argument (and every entry of an array of them) may be
+ *     pageable or pinned host memory, memory of any CUDA device, or managed memory; the checker libraries take host
+ *     memory.  Descriptors, options, arrays of pointers and scalar results are host memory.  The caller owns its
+ *     buffers; the library owns device memory inside DerpCtx.
  *   - images are row-major, top row first, tightly packed:
  *       colour  : uint16_t[H][W][3]  (B,G,R — cv::Vec3w, DerpUtil.h:19)
  *       float   : float[H][W]
@@ -145,8 +148,8 @@ int derp_get_sweep_stats(DerpCtx* ctx, uint64_t* refined, uint64_t* seeds);
  * (generateFovMasks, DerpUtil.cpp:259-276).  Invalidates everything from the previous level. */
 int derp_level_begin(DerpCtx* ctx, const DerpLevelParams* p);
 
-/* Source colours of all cameras, colors[s] = uint16_t[H][W][3] in host OR device memory (e.g. a level that
- * derp_downscale_area produced on the device); also computes the per-source
+/* Source colours of all cameras, colors[s] = uint16_t[H][W][3] (e.g. a level that derp_downscale_area produced on
+ * the device); also computes the per-source
  * variance (PyramidLevel::computeVariances PyramidLevel.h:232-247, computeImageVariance
  * DerpUtil.cpp:214-237). */
 int derp_set_colors(DerpCtx* ctx, const uint16_t* const* colors);
@@ -220,9 +223,7 @@ int derp_level_filter(DerpCtx* ctx, const DerpProcessOpts* opts);
  * (Derp.cpp:104-226) on interior pixels, NaN on the 1-px border.  Test/diagnostic entry. */
 int derp_eval_cost(DerpCtx* ctx, int dst, const float* disparity, float* out_cost, float* out_conf);
 
-/* Caller <-> context state. NULL pointers are skipped.  The disparity / cost / confidence planes of
- * derp_set_disparity and derp_get_disparity may live in host memory or in device memory (unified
- * addressing: the copy kind is inferred), so an exchange buffer of a collective can be filled directly. */
+/* Caller <-> context state. NULL pointers are skipped. */
 int derp_set_disparity(DerpCtx* ctx, int dst, const float* disparity, const float* cost,
                        const float* confidence);
 int derp_get_disparity(DerpCtx* ctx, int dst, float* disparity, float* cost, float* confidence);
@@ -272,15 +273,14 @@ int derp_device_copy(int device, void* dst, const void* src, size_t bytes);
 /* cv::resize(..., INTER_AREA) of a 3-channel 16-bit image, shrinking only: the resize scripts/render/resize.py:51-85
  * builds every pyramid level with (each level from the FULL-SIZE image, widths scripts/render/config.py:46), and the resize of
  * GenerateForegroundMasks' 16-bit inputs.  Bit-identical to OpenCV for integer
- * ratios (resizeAreaFast_) and general ratios (computeResizeAreaTab / ResizeArea_Invoker<ushort, float>).  src / dst may
- * be host or device memory. */
+ * ratios (resizeAreaFast_) and general ratios (computeResizeAreaTab / ResizeArea_Invoker<ushort, float>). */
 int derp_downscale_area(int device, const uint16_t* src, int src_w, int src_h, uint16_t* dst, int dst_w, int dst_h);
 
 /* generateForegroundMask<cv::Vec3w, cv::Vec3f> (source/render/BackgroundSubtractionUtil.h:20-59), the per-camera body of
  * the GenerateForegroundMasks app that produces the masks --use_foreground_masks consumes: Gaussian blur of template
  * (background) and frame (blur_radius 0 or 1 = the app's default 3 x 3 kernel), conversion to [0, 1] floats,
  * mask = ||template - frame||_2 > threshold, morphological closing with a morph_closing_size^2 rectangle.
- * Images u16 HxWx3 (host or device memory), mask uint8 HxW with values 0 / 1. */
+ * Images u16 HxWx3, mask uint8 HxW with values 0 / 1. */
 int derp_foreground_mask(int device, const uint16_t* templ, const uint16_t* frame, int width, int height, int blur_radius,
                          float threshold, int morph_closing_size, uint8_t* mask);
 
@@ -293,7 +293,7 @@ int derp_foreground_mask(int device, const uint16_t* templ, const uint16_t* fram
  * .vtx / .idx (MeshUtil.h:74-93): float32 x, y, z per vertex, uint32 x 3 per face, in the reference's order.
  * resolution_* / scalar_focal: the camera's (possibly rescaled, ConvertToBinary.cpp:322-343) resolution and
  * Camera::getScalarFocal().  `vertexes` needs room for 3 floats per grid cell, `faces` for 6 uint32 per grid cell
- * (derp_camera_mesh_size gives the grid); both may be host or device memory, like the inputs.
+ * (derp_camera_mesh_size gives the grid).
  * derp_camera_mesh_simplified adds the simplification step (ConvertToBinary.cpp:186-203): render::MeshSimplifier
  * (source/render/MeshSimplifier.cpp: quadric-error edge contraction, equi-error costs, strictness 0.2, boundary edges kept)
  * down to `triangles` faces when the mesh has more, then z < 0 -> FLT_MIN.  That stage is a chain of dependent
@@ -321,8 +321,7 @@ int derp_camera_mesh_simplified(int device, const float* disparity, int width, i
  * block loads through a lookup table over the stored channel values, built on the host with the host's powf.
  * Modes tried: 1 and 3 (best 3 / 1 of the 64 partitions by the residual bound), 6; same operation order, x86 conversion
  * semantics and end-point quantisation as the reference BUILD, IEEE division / square root where that build uses the
- * RCPPS / RSQRTPS estimates (so individual blocks can differ where an estimate's last bit decides; see derp_bc7.cuh).
- * All pointers may be host or device memory. */
+ * RCPPS / RSQRTPS estimates (so individual blocks can differ where an estimate's last bit decides; see derp_bc7.cuh). */
 int derp_bc7_compress(int device, const uint8_t* rgba, int width, int height, uint8_t* blocks);
 int derp_bc7_compress_image(int device, const void* pixels, int bits_per_channel, int channels, int width, int height,
                             float gamma, uint8_t* blocks);
