@@ -225,6 +225,9 @@ struct DerpCtx {
   size_t camSmem(int threads = kBlockX * kBlockY) const {
     return (size_t)S * sizeof(DevCamera) + kTileFloats * sizeof(float) + (size_t)selSlots() * threads * sizeof(float2);
   }
+  // the bound pass of the filtered sweep keeps no selection slots (KeptBound): S cameras + the destination tile, which
+  // leaves the rest of the SM's L1 to its gathers
+  size_t lowerSmem() const { return (size_t)S * sizeof(DevCamera) + kTileFloats * sizeof(float); }
   // compacted kernels: S cameras + one 3x3 patch per thread + the selection slots
   size_t patchSmem(int threads = kPatchThreads) const {
     return (size_t)S * sizeof(DevCamera) + (size_t)2 * 9 * threads * 2 * sizeof(float) + (size_t)selSlots() * threads * sizeof(float2);
@@ -765,7 +768,7 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
     LAUNCHED("fillKernel");
     CU(cudaMemsetAsync(c->dRefCount.p, 0, sizeof(unsigned long long), c->stream));
     const LowerArgs la = lowerArgs(c, dst, a.disparities, num_depths, chunk);
-    c->k.sweepLower<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), sweepSmem, c->stream>>>(la);
+    c->k.sweepLower<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), c->lowerSmem(), c->stream>>>(la);
     LAUNCHED("sweepLowerKernel");
     SeedArgs sa;
     sa.v = a.v;
@@ -1584,9 +1587,8 @@ int derp_debug_lower_bound(DerpCtx* c, int dst, int num_depths, float min_depth_
   if ((rc = resetCounters(c))) return rc;
   const LowerArgs la = lowerArgs(c, dst, dTab.p, num_depths, num_depths);
   const int by = kBlockY;
-  SMEM_FITS(c->camSmem(kBlockX * by), "sweepLowerKernel");
   SMEM_FITS(c->camSmem(), "lowerBoundCheckKernel");
-  c->k.sweepLower<<<dim3((W + kBlockX - 1) / kBlockX, (H + by - 1) / by, 1), dim3(kBlockX, by, 1), c->camSmem(kBlockX * by), c->stream>>>(la);
+  c->k.sweepLower<<<dim3((W + kBlockX - 1) / kBlockX, (H + by - 1) / by, 1), dim3(kBlockX, by, 1), c->lowerSmem(), c->stream>>>(la);
   LAUNCHED("sweepLowerKernel");
   CheckArgs ca;
   ca.v = la.v;
