@@ -133,6 +133,44 @@ struct UpsampleScratch {
   DevBuf<short2> spiral;
 };
 
+// CUDA events around launches on one stream, destroyed by clear() and the destructor: ev holds (start, stop) of every
+// logged launch, then the start of one in progress.  A launch that fails between begin() and end() is not counted: the
+// next begin() records over its start.
+struct EventLog {
+  std::vector<cudaEvent_t> ev;
+  EventLog() = default;
+  EventLog(const EventLog&) = delete;
+  EventLog& operator=(const EventLog&) = delete;
+  ~EventLog() { clear(); }
+  int begin(cudaStream_t st) { return ev.size() % 2 ? rerecord(st) : record(st); }
+  int end(cudaStream_t st) { return record(st); }
+  size_t count() const { return ev.size() / 2; }
+  // the summed device time of the logged launches; the stream must have been synchronised
+  int totalMs(double* ms) const {
+    *ms = 0;
+    for (size_t i = 0; i < 2 * count(); i += 2) {
+      float t = 0;
+      CU(cudaEventElapsedTime(&t, ev[i], ev[i + 1]));
+      *ms += t;
+    }
+    return DERP_OK;
+  }
+  void clear() {
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    ev.clear();
+  }
+  int record(cudaStream_t st) {
+    cudaEvent_t e;
+    CU(cudaEventCreate(&e));
+    ev.push_back(e);
+    return rerecord(st);
+  }
+  int rerecord(cudaStream_t st) {
+    CU(cudaEventRecord(ev.back(), st));
+    return DERP_OK;
+  }
+};
+
 }  // namespace
 
 struct DerpCtx {
@@ -191,33 +229,26 @@ struct DerpCtx {
   bool countersOnDevice = false;
   int tableD = -1;
   float tableMin = 0, tableMax = 0;  // candidate table currently in dDisparities
-  // optional per-kernel timing of the dominant kernel (sweepKernel) with CUDA events on c->stream
+  // optional timing of the brute-force sweeps and the pingPongKernel launches (derp_profile)
   bool profiling = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> sweepEvents;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pingEvents;  // pingPongKernel launches while profiling
-  DevBuf<unsigned long long> dCountersPP;                         // their own (evaluations, source hits)
+  EventLog sweepLog, pingLog;
+  DevBuf<unsigned long long> dCountersPP;  // the ping-pong launches' own (evaluations, source hits)
 
   float2* warpOf(int dst) const { return geomCached ? geom->buf.p + (size_t)dst * 2 * S * plane : dProjWarp.p; }
   float2* warpInvOf(int dst) const { return geomCached ? geom->buf.p + ((size_t)dst * 2 + 1) * S * plane : dWarpInv.p; }
-  const uint8_t* fgOf(int src) const { return haveFg ? dFg.p + (size_t)src * plane : nullptr; }
+  // the stages read the foreground mask (and the cost stages the background) only when the level uses foreground masks
+  const uint8_t* fgFor(int dst) const {
+    return lp.use_foreground_masks && haveFg ? dFg.p + (size_t)dst2src[dst] * plane : nullptr;
+  }
   const float* bgOf(int dst) const { return haveBg ? dBg.p + (size_t)dst * plane : nullptr; }
   CostView view(int dst) const {
-    CostView v;
-    v.W = W;
-    v.H = H;
-    v.S = S;
-    v.self = dst2src[dst];
-    v.projColor = dProjColor.p;
-    v.projBias = dProjBias.p;
-    v.projColor16 = dProjColor16.p;
-    v.projBias16 = dProjBias16.p;
-    v.selTab = dSelTab.p;
-    v.projWarp = warpOf(dst);
-    v.variance = dVariance.p + (size_t)v.self * plane;
-    v.cams = dCams.p;
-    v.one = 1.0f;
-    v.b23 = 8388608.0f;
-    return v;
+    const int self = dst2src[dst];
+    return CostView{W, H, S, self, dProjColor.p, dProjBias.p, dProjColor16.p, dProjBias16.p, dSelTab.p,
+                    warpOf(dst), dVariance.p + (size_t)self * plane, dCams.p, 1.0f, 8388608.0f};
+  }
+  // Call it after the stage's ensureTables*, which may reallocate the tables the view points at.
+  DstArgs dstArgs(int dst) const {
+    return DstArgs{view(dst), dFov.p + (size_t)dst * plane, fgFor(dst), lp.use_foreground_masks ? bgOf(dst) : nullptr};
   }
   // dynamic smem of the cost kernels: S cameras + the destination patch tile
   // + S - 1 (ssdB, ssdU) pairs per thread for the robust camera mean (one slot per possible source)
@@ -275,11 +306,6 @@ int checkSmem(size_t bytes, const char* what) {
   return fail(DERP_EINVAL, std::string(what) + ": needs " + std::to_string(bytes) + " B of shared memory per CTA, more than the " +
                                std::to_string(kMaxDynSmem) + " B an H100 grants");
 }
-#define SMEM_FITS(bytes, what)                \
-  do {                                        \
-    int rc_ = checkSmem(bytes, what);         \
-    if (rc_) return rc_;                      \
-  } while (0)
 
 int resetCounters(DerpCtx* c) {
   if (c->accumulateCounters) return DERP_OK;  // derp_level_estimate: one reset / one read-back for all stages
@@ -329,22 +355,149 @@ std::vector<float> probeDisparities(int num_depths, float min_depth_m, float max
   return disparities;
 }
 
-// arguments of sweepLowerKernel for one destination: bounds go to dLb, per-pixel seeds to dSeed
-LowerArgs lowerArgs(DerpCtx* c, int dst, const float* disparities, int num_depths, int chunk) {
-  const bool useFg = c->lp.use_foreground_masks != 0;
-  const int self = c->dst2src[dst];
-  LowerArgs la;
-  la.v = c->view(dst);
-  la.fov = c->dFov.p + (size_t)dst * c->plane;
-  la.fg = useFg ? c->fgOf(self) : nullptr;
-  la.bg = useFg ? c->bgOf(dst) : nullptr;
-  la.disparities = disparities;
-  la.D = num_depths;
-  la.chunk = chunk;
-  la.lb = c->dLb.p;
-  la.seed = c->dSeed.p;
-  la.counters = c->dCounters.p;
-  return la;
+int checkMasks(DerpCtx* c, const char* msg) {
+  if (c->lp.use_foreground_masks && (!c->haveBg || !c->haveFg)) return fail(DERP_ESTATE, msg);
+  return DERP_OK;
+}
+
+// Copies (to, from) between a caller's buffer and the context, returned with the copies done; a null end skips one
+int copyPlanes(DerpCtx* c, size_t bytes, std::initializer_list<std::pair<void*, const void*>> copies) {
+  for (const auto& p : copies)
+    if (p.first && p.second) CU(cudaMemcpyAsync(p.first, p.second, bytes, cudaMemcpyDefault, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return DERP_OK;
+}
+
+// The candidate table in dDisparities, uploaded only when it changes
+int candidateTable(DerpCtx* c, int num_depths, float min_depth_m, float max_depth_m) {
+  if (c->tableD == num_depths && c->tableMin == min_depth_m && c->tableMax == max_depth_m) return DERP_OK;
+  const std::vector<float> disparities = probeDisparities(num_depths, min_depth_m, max_depth_m);
+  if (int rc = upload(c->dDisparities, disparities.data(), num_depths, c->stream)) return rc;
+  CU(cudaStreamSynchronize(c->stream));  // host vector lifetime (tiny copy, only when the table changes)
+  c->tableD = num_depths;
+  c->tableMin = min_depth_m;
+  c->tableMax = max_depth_m;
+  return DERP_OK;
+}
+
+// Launch shape of sweepKernel and sweepLowerKernel: CTAs of kBlockX x rows threads, grid.z = chunks of `chunk` candidates
+struct SweepShape {
+  int rows, chunks, chunk;
+  dim3 grid(int W, int H) const { return dim3((W + kBlockX - 1) / kBlockX, (H + rows - 1) / rows, chunks); }
+};
+
+// CTA height: kSweepMaxRows rows (one 640-thread CTA per SM, 96 registers) on large levels — its warps share more texel
+// rows — and half of that (two CTAs per SM, same 20 warps) on small ones, where CTA count matters more.  Rigs of more
+// than 42 cameras get shorter CTAs (sweepRows).  Candidate chunks: enough CTAs to fill every SM with 8 resident CTAs
+// even on the coarse levels.
+SweepShape sweepShape(const DerpCtx* c, int num_depths) {
+  const int rows = c->sweepRows(c->H >= 1024 ? kSweepMaxRows : kSweepMaxRows / 2);
+  const long ctas = (long)((c->W + kBlockX - 1) / kBlockX) * ((c->H + rows - 1) / rows) * std::max(1, rows / 8);
+  const int chunks = (int)std::min<long>(num_depths, std::max<long>(1, ((long)c->numSMs * 8 * 4 + ctas - 1) / ctas));
+  const int chunk = (num_depths + chunks - 1) / chunks;
+  return SweepShape{rows, (num_depths + chunk - 1) / chunk, chunk};
+}
+
+// Filtered sweep (derp_refine.cuh) unless derp_set_sweep_mode chose the plain one, the candidate count is tiny or the
+// bound buffer does not fit: lower bound of every (pixel, candidate), exact cost only where the bound does not exclude
+// the candidate.  Automatic: the filter pays off when the bound pass amortises its extra launches and the read-back of
+// the list length: >= 32 M (pixel, candidate) pairs (512^2 x 128); BASELINE.json configs[0] (512^2 x 32) and the
+// coarsest pyramid levels stay on the plain sweep.
+bool useFilteredSweep(const DerpCtx* c, int num_depths, unsigned long long capacity) {
+  const int mode = c->sweepMode;
+  const size_t n = c->plane;
+  if (!(mode == 2 || (mode == 0 && num_depths >= 8 && (unsigned long long)n * (unsigned long long)num_depths >= (32ull << 20))))
+    return false;
+  size_t freeB = 0, totalB = 0;
+  cudaMemGetInfo(&freeB, &totalB);
+  const size_t need = (size_t)num_depths * n * sizeof(float) + capacity * sizeof(unsigned long long) + n * 8;
+  return !(c->dLb.n < (size_t)num_depths * n && need > freeB / 2);
+}
+
+// Pass 1 of the filtered sweep: the lower bound of every (pixel, candidate) into dLb, the per-pixel seeds into dSeed
+// (both allocated by the caller)
+int boundPass(DerpCtx* c, const DstArgs& da, const float* disparities, int num_depths, const SweepShape& shape) {
+  const size_t n = c->plane;
+  fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dSeed.p, 0x7f7fffffffffffffull);
+  LAUNCHED("fillKernel");
+  const LowerArgs la{da, disparities, num_depths, shape.chunk, c->dLb.p, c->dSeed.p, c->dCounters.p};
+  c->k.sweepLower<<<shape.grid(c->W, c->H), dim3(kBlockX, shape.rows), c->lowerSmem(), c->stream>>>(la);
+  LAUNCHED("sweepLowerKernel");
+  return DERP_OK;
+}
+
+// The filtered sweep into dBest: bound pass, seed, refine list, its length read back, refine.  *finished is false when
+// more candidates survived than the list holds (the bounds are useless on this input): dBest and the counters are then
+// reset for the plain sweep.
+int filteredSweep(DerpCtx* c, const DstArgs& da, int num_depths, const SweepShape& shape, unsigned long long capacity,
+                  bool* finished) {
+  const size_t n = c->plane;
+  CU(c->dLb.ensure((size_t)num_depths * n));
+  CU(c->dSeed.ensure(n));
+  CU(c->dRefList.ensure(capacity));
+  CU(c->dRefCount.ensure(1));
+  CU(cudaMemsetAsync(c->dRefCount.p, 0, sizeof(unsigned long long), c->stream));
+  int rc = boundPass(c, da, c->dDisparities.p, num_depths, shape);
+  if (rc) return rc;
+  const SeedArgs sa{da.v, da.fov, da.fg, c->dDisparities.p, c->dSeed.p, c->dBest.p};
+  c->k.sweepSeed<<<grid2(c->W, c->H), block2(), c->camSmem(), c->stream>>>(sa);
+  LAUNCHED("sweepSeedKernel");
+  const ListArgs li{c->W, c->H, num_depths, da.fov, da.fg, c->dLb.p, c->dSeed.p, c->dBest.p, c->dRefList.p, capacity,
+                    c->dRefCount.p};
+  refineListKernel<<<grid2(c->W, c->H), block2(), 0, c->stream>>>(li);
+  LAUNCHED("refineListKernel");
+  unsigned long long count = 0;
+  CU(cudaMemcpyAsync(&count, c->dRefCount.p, sizeof(count), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  *finished = count <= capacity;
+  if (!*finished) {
+    fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dBest.p, 0x7f7fffffffffffffull);
+    LAUNCHED("fillKernel");
+    CU(cudaMemsetAsync(c->dCounters.p, 0, 2 * sizeof(unsigned long long), c->stream));
+    return DERP_OK;
+  }
+  c->lastRefined = count;
+  c->lastSeeds = n;
+  if (count > 0) {
+    const RefineArgs ra{da.v, c->dDisparities.p, c->dRefList.p, count, c->dBest.p};
+    c->k.refine<<<(unsigned)((count + kPatchThreads - 1) / kPatchThreads), kPatchThreads, c->patchSmem(), c->stream>>>(ra);
+    LAUNCHED("refineKernel");
+  }
+  return DERP_OK;
+}
+
+int plainSweep(DerpCtx* c, const DstArgs& da, int num_depths, const SweepShape& shape) {
+  const SweepArgs a{da, c->dDisparities.p, num_depths, shape.chunk, c->dBest.p, c->dCounters.p};
+  c->k.sweep<<<shape.grid(c->W, c->H), dim3(kBlockX, shape.rows), c->camSmem(kBlockX * shape.rows), c->stream>>>(a);
+  LAUNCHED("sweepKernel");
+  return DERP_OK;
+}
+
+// dBest to the destination's disparity, cost and confidence with their borders extended; best_index (nullable) receives
+// the winning candidates.  Uncovered pixels fail the call unless partial_coverage or foreground masks allow them.
+int finishSweep(DerpCtx* c, int dst, const DstArgs& da, float minDisparity, int partial_coverage, int32_t* best_index) {
+  const int W = c->W, H = c->H;
+  const size_t n = c->plane;
+  float* disp = c->dDisp.p + (size_t)dst * n;
+  float* cost = c->dCost.p + (size_t)dst * n;
+  float* conf = c->dConf.p + (size_t)dst * n;
+  int* idx = best_index ? c->dIdx.p : nullptr;
+  sweepFinalizeKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, da.fov, da.fg, da.bg, da.v.variance, c->dDisparities.p,
+                                                               minDisparity, c->dBest.p, disp, cost, conf, idx, c->dUncovered.p);
+  LAUNCHED("sweepFinalizeKernel");
+  extendBorderKernel<<<grid1(2 * W + 2 * (H - 2)), 256, 0, c->stream>>>(W, H, da.fg, da.bg, disp, cost, conf, idx);
+  LAUNCHED("extendBorderKernel");
+  if (best_index) CU(cudaMemcpyAsync(best_index, c->dIdx.p, n * sizeof(int), cudaMemcpyDefault, c->stream));
+  if (!(partial_coverage || c->lp.use_foreground_masks)) {
+    unsigned unc = 0;
+    CU(cudaMemcpyAsync(&unc, c->dUncovered.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    if (unc > 0)  // Derp.cpp:339 CHECK(partialCoverage || useForegroundMasks)
+      return fail(DERP_ECOVERAGE, "Insufficient coverage at " + std::to_string(unc) + " pixels");
+  } else if (best_index) {
+    CU(cudaStreamSynchronize(c->stream));
+  }
+  return DERP_OK;
 }
 
 }  // namespace
@@ -399,15 +552,10 @@ int derp_create(const DerpCameraDesc* cams, int num_cams, const int32_t* dst_to_
   // the cost kernels keep cameras, the destination patch tile / per-thread patches and the selection slots in
   // dynamic shared memory: 92 KB for a 640-thread sweep CTA of a 16-camera rig, 177 KB with 32 cameras, 216 KB for a
   // 384-thread one with 64 cameras (DerpCtx::sweepRows); kMaxDynSmem is the most an H100 grants one CTA
-  const int maxSmem = (int)kMaxDynSmem;
-  CU(cudaFuncSetAttribute(c->k.sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.evalCost, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.proposal, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.pingPong, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.sweepLower, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.sweepSeed, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.refine, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
-  CU(cudaFuncSetAttribute(c->k.lowerBoundCheck, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem));
+  const CostKernels& k = c->k;
+  for (const void* f : {(const void*)k.sweep, (const void*)k.evalCost, (const void*)k.proposal, (const void*)k.pingPong,
+                        (const void*)k.sweepLower, (const void*)k.sweepSeed, (const void*)k.refine, (const void*)k.lowerBoundCheck})
+    CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
   *out = c.release();
   return DERP_OK;
 }
@@ -420,17 +568,6 @@ void derp_destroy(DerpCtx* c) {
   delete c;
 }
 
-int derp_set_stream(DerpCtx* c, void* cuda_stream) {
-  if (!c) return fail(DERP_EINVAL, "null ctx");
-  int rc = useDevice(c);
-  if (rc) return rc;
-  CU(cudaStreamSynchronize(c->stream));
-  if (c->ownStream && c->stream) cudaStreamDestroy(c->stream);
-  c->ownStream = false;
-  c->stream = (cudaStream_t)cuda_stream;
-  return DERP_OK;
-}
-
 int derp_sync(DerpCtx* c) {
   if (!c) return fail(DERP_EINVAL, "null ctx");
   int rc = useDevice(c);
@@ -439,18 +576,18 @@ int derp_sync(DerpCtx* c) {
   return DERP_OK;
 }
 
+int derp_set_stream(DerpCtx* c, void* cuda_stream) {
+  if (int rc = derp_sync(c)) return rc;
+  if (c->ownStream && c->stream) cudaStreamDestroy(c->stream);
+  c->ownStream = false;
+  c->stream = (cudaStream_t)cuda_stream;
+  return DERP_OK;
+}
+
 int derp_profile(DerpCtx* c, int enable) {
   if (!c) return fail(DERP_EINVAL, "null ctx");
-  for (auto& e : c->sweepEvents) {
-    cudaEventDestroy(e.first);
-    cudaEventDestroy(e.second);
-  }
-  c->sweepEvents.clear();
-  for (auto& e : c->pingEvents) {
-    cudaEventDestroy(e.first);
-    cudaEventDestroy(e.second);
-  }
-  c->pingEvents.clear();
+  c->sweepLog.clear();
+  c->pingLog.clear();
   c->profiling = enable != 0;
   if (c->profiling) {
     CU(c->dCountersPP.ensure(2));
@@ -460,38 +597,26 @@ int derp_profile(DerpCtx* c, int enable) {
 }
 
 int derp_get_profile_ping_pong(DerpCtx* c, double* ms, uint64_t* launches, uint64_t* evals, uint64_t* hits) {
-  if (!c) return fail(DERP_EINVAL, "null ctx");
-  int rc = useDevice(c);
+  int rc = derp_sync(c);
   if (rc) return rc;
-  CU(cudaStreamSynchronize(c->stream));
   double total = 0;
-  for (auto& e : c->pingEvents) {
-    float t = 0;
-    CU(cudaEventElapsedTime(&t, e.first, e.second));
-    total += t;
-  }
+  if ((rc = c->pingLog.totalMs(&total))) return rc;
   unsigned long long h[2] = {0, 0};
   if (c->dCountersPP.p) CU(cudaMemcpy(h, c->dCountersPP.p, sizeof(h), cudaMemcpyDeviceToHost));
   if (ms) *ms = total;
-  if (launches) *launches = c->pingEvents.size();
+  if (launches) *launches = c->pingLog.count();
   if (evals) *evals = h[0];
   if (hits) *hits = h[1];
   return DERP_OK;
 }
 
 int derp_get_profile(DerpCtx* c, double* sweep_ms, uint64_t* sweep_launches) {
-  if (!c) return fail(DERP_EINVAL, "null ctx");
-  int rc = useDevice(c);
+  int rc = derp_sync(c);
   if (rc) return rc;
-  CU(cudaStreamSynchronize(c->stream));
   double total = 0;
-  for (auto& e : c->sweepEvents) {
-    float ms = 0;
-    CU(cudaEventElapsedTime(&ms, e.first, e.second));
-    total += ms;
-  }
+  if ((rc = c->sweepLog.totalMs(&total))) return rc;
   if (sweep_ms) *sweep_ms = total;
-  if (sweep_launches) *sweep_launches = c->sweepEvents.size();
+  if (sweep_launches) *sweep_launches = c->sweepLog.count();
   return DERP_OK;
 }
 
@@ -676,7 +801,7 @@ int derp_eval_cost(DerpCtx* c, int dst, const float* disparity, float* out_cost,
   CU(cudaMemcpyAsync(c->dScratchA.p, disparity, n * sizeof(float), cudaMemcpyDefault, c->stream));
   if ((rc = resetCounters(c))) return rc;
   if ((rc = ensureTablesF32(c))) return rc;
-  SMEM_FITS(c->camSmem(), "evalCostKernel");
+  if ((rc = checkSmem(c->camSmem(), "evalCostKernel"))) return rc;
   c->k.evalCost<<<grid2(c->W, c->H), block2(), c->camSmem(), c->stream>>>(c->view(dst), c->dScratchA.p, c->dScratchB.p,
                                                                          c->dScratchC.p, c->dCounters.p);
   LAUNCHED("evalCostKernel");
@@ -692,198 +817,51 @@ int derp_brute_force(DerpCtx* c, int dst, int num_depths, float min_depth_m, flo
   if (num_depths < 2) return fail(DERP_EINVAL, "derp_brute_force: bad arguments");
   int rc = checkDst(c, dst, "derp_brute_force", true);
   if (rc) return rc;
-  const bool useFg = c->lp.use_foreground_masks != 0;
-  if (useFg && (!c->haveBg || !c->haveFg))
-    return fail(DERP_ESTATE, "derp_brute_force: foreground masks / background disparity not set");
-  const int W = c->W, H = c->H;
-  const size_t n = c->plane;
-  const int self = c->dst2src[dst];
-  const float minDisparity = 1.0f / max_depth_m;
-  if (c->tableD != num_depths || c->tableMin != min_depth_m || c->tableMax != max_depth_m) {
-    const std::vector<float> disparities = probeDisparities(num_depths, min_depth_m, max_depth_m);
-    if ((rc = upload(c->dDisparities, disparities.data(), num_depths, c->stream))) return rc;
-    CU(cudaStreamSynchronize(c->stream));  // host vector lifetime (tiny copy, only when the table changes)
-    c->tableD = num_depths;
-    c->tableMin = min_depth_m;
-    c->tableMax = max_depth_m;
-  }
+  if ((rc = checkMasks(c, "derp_brute_force: foreground masks / background disparity not set"))) return rc;
+  if ((rc = candidateTable(c, num_depths, min_depth_m, max_depth_m))) return rc;
   if ((rc = ensureTablesF32(c))) return rc;
+  const size_t n = c->plane;
   fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dBest.p, 0x7f7fffffffffffffull);
   LAUNCHED("fillKernel");
   if ((rc = resetCounters(c))) return rc;
   CU(cudaMemsetAsync(c->dUncovered.p, 0, sizeof(unsigned), c->stream));
-  // candidate chunks: enough CTAs to fill every SM with 8 resident CTAs even on the coarse levels
-  // CTA height of the sweep: kSweepMaxRows rows (one 640-thread CTA per SM, 96 registers) on large levels —
-  // its warps share more texel rows — and half of that (two CTAs per SM, same 20 warps) on small ones, where CTA count matters
-  // more.  Rigs of more than 42 cameras get shorter CTAs (sweepRows).
-  const int sweepBY = c->sweepRows(H >= 1024 ? kSweepMaxRows : kSweepMaxRows / 2);
-  const size_t sweepSmem = c->camSmem(kBlockX * sweepBY);
-  SMEM_FITS(sweepSmem, "sweepKernel");
-  SMEM_FITS(c->camSmem(), "sweepSeedKernel");
-  SMEM_FITS(c->patchSmem(), "refineKernel");
-  const dim3 g = grid2(W, H);
-  const dim3 gs((W + kBlockX - 1) / kBlockX, (H + sweepBY - 1) / sweepBY, 1);
-  const long ctas = (long)gs.x * gs.y * std::max(1, sweepBY / 8);
-  int chunks = (int)std::min<long>(num_depths, std::max<long>(1, ((long)c->numSMs * 8 * 4 + ctas - 1) / ctas));
-  const int chunk = (num_depths + chunks - 1) / chunks;
-  chunks = (num_depths + chunk - 1) / chunk;
-  SweepArgs a;
-  a.v = c->view(dst);
-  a.fov = c->dFov.p + (size_t)dst * n;
-  a.fg = useFg ? c->fgOf(self) : nullptr;
-  a.bg = useFg ? c->bgOf(dst) : nullptr;
-  a.disparities = c->dDisparities.p;
-  a.D = num_depths;
-  a.chunk = chunk;
-  a.best = c->dBest.p;
-  a.counters = c->dCounters.p;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  if (c->profiling) {
-    CU(cudaEventCreate(&ev0));
-    CU(cudaEventCreate(&ev1));
-    CU(cudaEventRecord(ev0, c->stream));
-  }
-  // Filtered sweep (derp_refine.cuh) unless derp_set_sweep_mode chose the plain one, the candidate count is tiny or the
-  // bound buffer does not fit: lower bound of every (pixel, candidate), exact cost only where the bound does not exclude
-  // the candidate.
-  const int mode = c->sweepMode;
-  // automatic: the filter pays off when the bound pass amortises its extra launches and the read-back of the list
-  // length: >= 32 M (pixel, candidate) pairs (512^2 x 128); BASELINE.json configs[0] (512^2 x 32) and the coarsest
-  // pyramid levels stay on the plain sweep
-  bool filtered = mode == 2 || (mode == 0 && num_depths >= 8 && (unsigned long long)n * (unsigned long long)num_depths >= (32ull << 20));
-  const unsigned long long capacity = (unsigned long long)n * (unsigned long long)std::max(2, num_depths / 8);
-  if (filtered) {
-    size_t freeB = 0, totalB = 0;
-    cudaMemGetInfo(&freeB, &totalB);
-    const size_t need = (size_t)num_depths * n * sizeof(float) + capacity * sizeof(unsigned long long) + n * 8;
-    if (c->dLb.n < (size_t)num_depths * n && need > freeB / 2) filtered = false;
-  }
+  const SweepShape shape = sweepShape(c, num_depths);
+  if ((rc = checkSmem(c->camSmem(kBlockX * shape.rows), "sweepKernel"))) return rc;
+  if ((rc = checkSmem(c->camSmem(), "sweepSeedKernel"))) return rc;
+  if ((rc = checkSmem(c->patchSmem(), "refineKernel"))) return rc;
+  const DstArgs da = c->dstArgs(dst);  // after ensureTablesF32 (see dstArgs)
+  if (c->profiling && (rc = c->sweepLog.begin(c->stream))) return rc;
   c->lastRefined = c->lastSeeds = 0;
-  if (filtered) {
-    CU(c->dLb.ensure((size_t)num_depths * n));
-    CU(c->dSeed.ensure(n));
-    CU(c->dRefList.ensure(capacity));
-    CU(c->dRefCount.ensure(1));
-    fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dSeed.p, 0x7f7fffffffffffffull);
-    LAUNCHED("fillKernel");
-    CU(cudaMemsetAsync(c->dRefCount.p, 0, sizeof(unsigned long long), c->stream));
-    const LowerArgs la = lowerArgs(c, dst, a.disparities, num_depths, chunk);
-    c->k.sweepLower<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), c->lowerSmem(), c->stream>>>(la);
-    LAUNCHED("sweepLowerKernel");
-    SeedArgs sa;
-    sa.v = a.v;
-    sa.fov = a.fov;
-    sa.fg = a.fg;
-    sa.disparities = a.disparities;
-    sa.seed = c->dSeed.p;
-    sa.best = c->dBest.p;
-    c->k.sweepSeed<<<g, block2(), c->camSmem(), c->stream>>>(sa);
-    LAUNCHED("sweepSeedKernel");
-    ListArgs li;
-    li.W = W;
-    li.H = H;
-    li.D = num_depths;
-    li.fov = a.fov;
-    li.fg = a.fg;
-    li.lb = c->dLb.p;
-    li.seed = c->dSeed.p;
-    li.best = c->dBest.p;
-    li.list = c->dRefList.p;
-    li.capacity = capacity;
-    li.count = c->dRefCount.p;
-    refineListKernel<<<g, block2(), 0, c->stream>>>(li);
-    LAUNCHED("refineListKernel");
-    unsigned long long count = 0;
-    CU(cudaMemcpyAsync(&count, c->dRefCount.p, sizeof(count), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    if (count > capacity) {
-      // more survivors than the list holds (bounds useless on this input): redo the destination with the plain sweep
-      filtered = false;
-      fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dBest.p, 0x7f7fffffffffffffull);
-      LAUNCHED("fillKernel");
-      CU(cudaMemsetAsync(c->dCounters.p, 0, 2 * sizeof(unsigned long long), c->stream));
-    } else {
-      c->lastRefined = count;
-      c->lastSeeds = n;
-      if (count > 0) {
-        RefineArgs ra;
-        ra.v = a.v;
-        ra.disparities = a.disparities;
-        ra.list = c->dRefList.p;
-        ra.count = count;
-        ra.best = c->dBest.p;
-        c->k.refine<<<(unsigned)((count + kPatchThreads - 1) / kPatchThreads), kPatchThreads, c->patchSmem(), c->stream>>>(ra);
-        LAUNCHED("refineKernel");
-      }
-    }
-  }
-  if (!filtered) {
-    c->k.sweep<<<dim3(gs.x, gs.y, chunks), dim3(kBlockX, sweepBY, 1), sweepSmem, c->stream>>>(a);
-    LAUNCHED("sweepKernel");
-  }
-  if (c->profiling) {
-    CU(cudaEventRecord(ev1, c->stream));
-    c->sweepEvents.emplace_back(ev0, ev1);
-  }
-  float* disp = c->dDisp.p + (size_t)dst * n;
-  float* cost = c->dCost.p + (size_t)dst * n;
-  float* conf = c->dConf.p + (size_t)dst * n;
-  int* idx = best_index ? c->dIdx.p : nullptr;
-  sweepFinalizeKernel<<<g, block2(), 0, c->stream>>>(W, H, a.fov, a.fg, a.bg, a.v.variance, c->dDisparities.p, minDisparity,
-                                                     c->dBest.p, disp, cost, conf, idx, c->dUncovered.p);
-  LAUNCHED("sweepFinalizeKernel");
-  extendBorderKernel<<<grid1(2 * W + 2 * (H - 2)), 256, 0, c->stream>>>(W, H, a.fg, a.bg, disp, cost, conf, idx);
-  LAUNCHED("extendBorderKernel");
-  if (best_index) CU(cudaMemcpyAsync(best_index, c->dIdx.p, n * sizeof(int), cudaMemcpyDefault, c->stream));
-  if (!(partial_coverage || useFg)) {
-    unsigned unc = 0;
-    CU(cudaMemcpyAsync(&unc, c->dUncovered.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    if (unc > 0)  // Derp.cpp:339 CHECK(partialCoverage || useForegroundMasks)
-      return fail(DERP_ECOVERAGE, "Insufficient coverage at " + std::to_string(unc) + " pixels");
-  } else if (best_index) {
-    CU(cudaStreamSynchronize(c->stream));
-  }
-  return DERP_OK;
+  const unsigned long long capacity = (unsigned long long)n * std::max(2, num_depths / 8);  // refine list entries
+  bool finished = false;
+  if (useFilteredSweep(c, num_depths, capacity) && (rc = filteredSweep(c, da, num_depths, shape, capacity, &finished)))
+    return rc;
+  if (!finished && (rc = plainSweep(c, da, num_depths, shape))) return rc;
+  if (c->profiling && (rc = c->sweepLog.end(c->stream))) return rc;
+  return finishSweep(c, dst, da, 1.0f / max_depth_m, partial_coverage, best_index);
 }
 
 int derp_random_proposals(DerpCtx* c, int dst, int num_proposals, float min_depth_m, float max_depth_m) {
   int rc = checkDst(c, dst, "derp_random_proposals", true);
   if (rc) return rc;
   if (num_proposals < 0) return fail(DERP_EINVAL, "derp_random_proposals: negative count");
-  const bool useFg = c->lp.use_foreground_masks != 0;
-  if (useFg && (!c->haveBg || !c->haveFg)) return fail(DERP_ESTATE, "derp_random_proposals: masks not set");
+  if ((rc = checkMasks(c, "derp_random_proposals: masks not set"))) return rc;
   const int W = c->W, H = c->H;
   const size_t n = c->plane;
-  const int self = c->dst2src[dst];
   const float kRandomPropHighVarDeviation = 0.1f;  // Derp.h:37
   const float varHighDev = kRandomPropHighVarDeviation * c->lp.var_high_thresh;
   const float varThresh = std::max(varHighDev, c->varNoiseFloor);
-  ProposalArgs a;
-  a.v = c->view(dst);
-  a.fov = c->dFov.p + (size_t)dst * n;
-  a.fg = useFg ? c->fgOf(self) : nullptr;
-  a.bg = useFg ? c->bgOf(dst) : nullptr;
-  a.prefix = c->dPrefix.p;
-  a.disp = c->dDisp.p + (size_t)dst * n;
-  a.cost = c->dCost.p + (size_t)dst * n;
-  a.conf = c->dConf.p + (size_t)dst * n;
-  a.numProposals = num_proposals;
-  a.level = c->lp.level;
-  a.minDispGlobal = 1.0f / max_depth_m;
-  a.maxDisp = 1.0f / min_depth_m;
-  a.counters = c->dCounters.p;
-  a.list = c->dList.p;
-  a.listCount = listCountPtr(c);
   if ((rc = resetCounters(c))) return rc;
   if ((rc = ensureTablesU16(c))) return rc;
-  a.v = c->view(dst);  // the u16 tables may just have been allocated
+  const size_t o = (size_t)dst * n;  // dstArgs after ensureTablesU16 (see dstArgs)
+  const ProposalArgs a{c->dstArgs(dst), c->dPrefix.p, c->dList.p, listCountPtr(c), c->dDisp.p + o, c->dCost.p + o,
+                       c->dConf.p + o, num_proposals, c->lp.level, 1.0f / max_depth_m, 1.0f / min_depth_m, c->dCounters.p};
   if ((rc = buildActiveList(c, a.fov, a.fg, a.v.variance, varThresh))) return rc;
-  if (useFg) {
+  if (c->lp.use_foreground_masks) {
     backgroundFillKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, a.fov, a.fg, a.bg, a.disp);
     LAUNCHED("backgroundFillKernel");
   }
-  SMEM_FITS(c->patchSmem(), "proposalKernel");
+  if ((rc = checkSmem(c->patchSmem(), "proposalKernel"))) return rc;
   c->k.proposal<<<listGrid(W, H), kPatchThreads, c->patchSmem(), c->stream>>>(a);
   LAUNCHED("proposalKernel");
   return DERP_OK;
@@ -892,54 +870,33 @@ int derp_random_proposals(DerpCtx* c, int dst, int num_proposals, float min_dept
 int derp_ping_pong(DerpCtx* c, int dst, int iterations) {
   int rc = checkDst(c, dst, "derp_ping_pong", true);
   if (rc) return rc;
-  const bool useFg = c->lp.use_foreground_masks != 0;
-  if (useFg && (!c->haveBg || !c->haveFg)) return fail(DERP_ESTATE, "derp_ping_pong: masks not set");
+  if ((rc = checkMasks(c, "derp_ping_pong: masks not set"))) return rc;
   const int W = c->W, H = c->H;
   const size_t n = c->plane;
-  const int self = c->dst2src[dst];
   float* disp = c->dDisp.p + (size_t)dst * n;
   float* cost = c->dCost.p + (size_t)dst * n;
-  const uint8_t* fov = c->dFov.p + (size_t)dst * n;
-  const uint8_t* fg = useFg ? c->fgOf(self) : nullptr;
-  const float* bg = useFg ? c->bgOf(dst) : nullptr;
   if ((rc = resetCounters(c))) return rc;
   if ((rc = ensureTablesU16(c))) return rc;
+  // dstArgs after ensureTablesU16 (see dstArgs); changed / changedNext are set per iteration
+  PingPongArgs a{c->dstArgs(dst), disp, nullptr, c->dScratchA.p, c->dScratchB.p, nullptr, c->dList.p, listCountPtr(c),
+                 c->dCounters.p, c->profiling ? c->dCountersPP.p : nullptr};
   // active pixels: interior, in FOV, foreground, variance >= noise floor (Derp.cpp:420-437)
-  if ((rc = buildActiveList(c, fov, fg, c->view(dst).variance, c->varNoiseFloor))) return rc;
+  if ((rc = buildActiveList(c, a.fov, a.fg, a.v.variance, c->varNoiseFloor))) return rc;
   fillKernel<uint8_t><<<grid1(n), 256, 0, c->stream>>>(n, c->dChangedA.p, (uint8_t)1);
   LAUNCHED("fillKernel");
   uint8_t* chIn = c->dChangedA.p;
   uint8_t* chOut = c->dChangedB.p;
-  SMEM_FITS(c->patchSmem(kPingThreads), "pingPongKernel");
+  if ((rc = checkSmem(c->patchSmem(kPingThreads), "pingPongKernel"))) return rc;
   for (int it = 1; it <= iterations; ++it) {
-    pingPongInitKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, fov, fg, bg, disp, c->dScratchA.p, c->dScratchB.p, chOut);
+    pingPongInitKernel<<<grid2(W, H), block2(), 0, c->stream>>>(W, H, a.fov, a.fg, a.bg, disp, c->dScratchA.p, c->dScratchB.p,
+                                                                chOut);
     LAUNCHED("pingPongInitKernel");
-    PingPongArgs a;
-    a.v = c->view(dst);
-    a.fov = fov;
-    a.fg = fg;
-    a.bg = bg;
-    a.disp = disp;
     a.changed = chIn;
-    a.dispRes = c->dScratchA.p;
-    a.costRes = c->dScratchB.p;
     a.changedNext = chOut;
-    a.list = c->dList.p;
-    a.listCount = listCountPtr(c);
-    a.counters = c->dCounters.p;
-    a.counters2 = c->profiling ? c->dCountersPP.p : nullptr;
-    cudaEvent_t p0 = nullptr, p1 = nullptr;
-    if (c->profiling) {
-      CU(cudaEventCreate(&p0));
-      CU(cudaEventCreate(&p1));
-      CU(cudaEventRecord(p0, c->stream));
-    }
+    if (c->profiling && (rc = c->pingLog.begin(c->stream))) return rc;
     c->k.pingPong<<<listGrid(W, H, kPingThreads), kPingThreads, c->patchSmem(kPingThreads), c->stream>>>(a);
     LAUNCHED("pingPongKernel");
-    if (c->profiling) {
-      CU(cudaEventRecord(p1, c->stream));
-      c->pingEvents.emplace_back(p0, p1);
-    }
+    if (c->profiling && (rc = c->pingLog.end(c->stream))) return rc;
     // disp <- dispRes, cost <- costsRes (Derp.cpp:527-529); confidence is not written back
     CU(cudaMemcpyAsync(disp, c->dScratchA.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
     CU(cudaMemcpyAsync(cost, c->dScratchB.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
@@ -954,20 +911,9 @@ static int launchMismatches(DerpCtx* c, const float* dispAll) {
   CU(c->dDispNext.ensure(n * c->Sd));
   for (int d = 0; d < c->Sd; ++d) {
     const int self = c->dst2src[d];
-    MismatchArgs a;
-    a.W = c->W;
-    a.H = c->H;
-    a.S = c->S;
-    a.self = self;
-    a.cams = c->dCams.p;
-    a.dispAll = dispAll;
-    a.variance = c->dVariance.p + (size_t)self * n;
-    a.fov = c->dFov.p + (size_t)d * n;
-    a.fg = (c->lp.use_foreground_masks && c->haveFg) ? c->fgOf(self) : nullptr;
-    a.varNoiseFloor = c->varNoiseFloor;
-    a.varHighThresh = c->lp.var_high_thresh;
-    a.dispNew = c->dDispNext.p + (size_t)d * n;
-    a.mask = c->dMismatch.p + (size_t)d * n;
+    const MismatchArgs a{c->W, c->H, c->S, self, c->dCams.p, dispAll, c->dVariance.p + (size_t)self * n, c->dFov.p + (size_t)d * n,
+                         c->fgFor(d), c->varNoiseFloor, c->lp.var_high_thresh, c->dDispNext.p + (size_t)d * n,
+                         c->dMismatch.p + (size_t)d * n};
     mismatchKernel<<<grid2(c->W, c->H), block2(), (size_t)c->S * sizeof(DevCamera), c->stream>>>(a);  // cameras only
     LAUNCHED("mismatchKernel");
   }
@@ -1045,15 +991,14 @@ int derp_bilateral(DerpCtx* c, int dst) {
   // Derp.cpp:876-878: pow(float, int) promotes to double, result narrowed to float
   const float scale = (float)std::pow((double)0.9f, (double)c->lp.level);
   const int spaceRadius = (int)std::max(std::ceil(5 * scale), float(1));
-  const uint8_t* fg = (c->lp.use_foreground_masks && c->haveFg) ? c->fgOf(self) : nullptr;
   float* disp = c->dDisp.p + (size_t)dst * n;
   const float sigma = 0.005f;
   DivConst three, denom;
   CU(makeDivConst(3.0f, c->stream, &three));
   CU(makeDivConst(2.0f * (sigma * sigma), c->stream, &denom));
   bilateralKernel<GuideU16><<<grid2(c->W, c->H), block2(), bilateralSmem(spaceRadius), c->stream>>>(
-      c->W, c->H, disp, GuideU16{c->dColor.p + (size_t)self * n}, c->dFov.p + (size_t)dst * n, fg, spaceRadius, three, denom,
-      0.5f, 1.0f, 1.0f, c->dScratchA.p);
+      c->W, c->H, disp, GuideU16{c->dColor.p + (size_t)self * n}, c->dFov.p + (size_t)dst * n, c->fgFor(dst), spaceRadius,
+      three, denom, 0.5f, 1.0f, 1.0f, c->dScratchA.p);
   LAUNCHED("bilateralKernel");
   CU(cudaMemcpyAsync(disp, c->dScratchA.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   return DERP_OK;
@@ -1063,11 +1008,11 @@ int derp_median(DerpCtx* c, int dst) {
   int rc = checkDst(c, dst, "derp_median", false);
   if (rc) return rc;
   const size_t n = c->plane;
-  const int self = c->dst2src[dst];
-  const uint8_t* fg = (c->lp.use_foreground_masks && c->haveFg) ? c->fgOf(self) : nullptr;
   float* disp = c->dDisp.p + (size_t)dst * n;
-  medianKernel<<<grid2(c->W, c->H), block2(), 0, c->stream>>>(c->W, c->H, disp, c->bgOf(dst), c->dFov.p + (size_t)dst * n, fg,
-                                                             c->dScratchA.p);
+  // The background is passed whenever one is set, also with use_foreground_masks off (unlike dstArgs' background), and
+  // the kernel writes it to every pixel outside the FOV (and foreground) mask.
+  medianKernel<<<grid2(c->W, c->H), block2(), 0, c->stream>>>(c->W, c->H, disp, c->bgOf(dst), c->dFov.p + (size_t)dst * n,
+                                                             c->fgFor(dst), c->dScratchA.p);
   LAUNCHED("medianKernel");
   CU(cudaMemcpyAsync(disp, c->dScratchA.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   return DERP_OK;
@@ -1440,42 +1385,28 @@ int derp_process_level(DerpCtx* c, const DerpProcessOpts* o) {
 int derp_set_disparity(DerpCtx* c, int dst, const float* disparity, const float* cost, const float* confidence) {
   int rc = checkDst(c, dst, "derp_set_disparity", false);
   if (rc) return rc;
-  const size_t n = c->plane, b = n * sizeof(float);
-  if (disparity) CU(cudaMemcpyAsync(c->dDisp.p + (size_t)dst * n, disparity, b, cudaMemcpyDefault, c->stream));
-  if (cost) CU(cudaMemcpyAsync(c->dCost.p + (size_t)dst * n, cost, b, cudaMemcpyDefault, c->stream));
-  if (confidence) CU(cudaMemcpyAsync(c->dConf.p + (size_t)dst * n, confidence, b, cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  const size_t n = c->plane;
+  return copyPlanes(c, n * sizeof(float), {{c->dDisp.p + (size_t)dst * n, disparity}, {c->dCost.p + (size_t)dst * n, cost},
+                                           {c->dConf.p + (size_t)dst * n, confidence}});
 }
 
 int derp_get_disparity(DerpCtx* c, int dst, float* disparity, float* cost, float* confidence) {
   int rc = checkDst(c, dst, "derp_get_disparity", false);
   if (rc) return rc;
-  const size_t n = c->plane, b = n * sizeof(float);
-  if (disparity) CU(cudaMemcpyAsync(disparity, c->dDisp.p + (size_t)dst * n, b, cudaMemcpyDefault, c->stream));
-  if (cost) CU(cudaMemcpyAsync(cost, c->dCost.p + (size_t)dst * n, b, cudaMemcpyDefault, c->stream));
-  if (confidence) CU(cudaMemcpyAsync(confidence, c->dConf.p + (size_t)dst * n, b, cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  const size_t n = c->plane;
+  return copyPlanes(c, n * sizeof(float), {{disparity, c->dDisp.p + (size_t)dst * n}, {cost, c->dCost.p + (size_t)dst * n},
+                                           {confidence, c->dConf.p + (size_t)dst * n}});
 }
 
-int derp_get_fov_mask(DerpCtx* c, int dst, uint8_t* mask) {
+// destination dst's plane of the FOV or the mismatch masks
+static int getMask(DerpCtx* c, int dst, uint8_t* mask, const char* who, bool mismatch) {
   if (!mask) return fail(DERP_EINVAL, "bad arguments");
-  int rc = checkDst(c, dst, "derp_get_fov_mask", false);
+  int rc = checkDst(c, dst, who, false);
   if (rc) return rc;
-  CU(cudaMemcpyAsync(mask, c->dFov.p + (size_t)dst * c->plane, c->plane, cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  return copyPlanes(c, c->plane, {{mask, (mismatch ? c->dMismatch.p : c->dFov.p) + (size_t)dst * c->plane}});
 }
-
-int derp_get_mismatch_mask(DerpCtx* c, int dst, uint8_t* mask) {
-  if (!mask) return fail(DERP_EINVAL, "bad arguments");
-  int rc = checkDst(c, dst, "derp_get_mismatch_mask", false);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(mask, c->dMismatch.p + (size_t)dst * c->plane, c->plane, cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
-}
+int derp_get_fov_mask(DerpCtx* c, int dst, uint8_t* mask) { return getMask(c, dst, mask, "derp_get_fov_mask", false); }
+int derp_get_mismatch_mask(DerpCtx* c, int dst, uint8_t* mask) { return getMask(c, dst, mask, "derp_get_mismatch_mask", true); }
 
 int derp_get_variance(DerpCtx* c, int src, float* variance) {
   if (!c || !variance) return fail(DERP_EINVAL, "bad arguments");
@@ -1483,9 +1414,7 @@ int derp_get_variance(DerpCtx* c, int src, float* variance) {
   if (src < 0 || src >= c->S) return fail(DERP_EINVAL, "src out of range");
   int rc = useDevice(c);
   if (rc) return rc;
-  CU(cudaMemcpyAsync(variance, c->dVariance.p + (size_t)src * c->plane, c->plane * sizeof(float), cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  return copyPlanes(c, c->plane * sizeof(float), {{variance, c->dVariance.p + (size_t)src * c->plane}});
 }
 
 int derp_get_var_noise_floor(DerpCtx* c, float* out) {
@@ -1505,36 +1434,23 @@ int derp_get_proj_warp(DerpCtx* c, int src, float* warp_xy) {
   if (!warp_xy) return fail(DERP_EINVAL, "bad arguments");
   int rc = checkProj(c, src, "derp_get_proj_warp");
   if (rc) return rc;
-  CU(cudaMemcpyAsync(warp_xy, c->warpOf(c->projDst) + (size_t)src * c->plane, c->plane * sizeof(float2), cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  return copyPlanes(c, c->plane * sizeof(float2), {{warp_xy, c->warpOf(c->projDst) + (size_t)src * c->plane}});
 }
 
-static int getTexels(DerpCtx* c, const float4* plane, uint16_t* bgr) {
+// source src's plane of the float4 colour or bias table as u16 B, G, R texels
+static int getTexels(DerpCtx* c, int src, uint16_t* bgr, const char* who, bool bias) {
+  if (!bgr) return fail(DERP_EINVAL, "bad arguments");
+  int rc = checkProj(c, src, who);
+  if (rc) return rc;
+  if ((rc = ensureTablesF32(c))) return rc;  // may reallocate the tables
   const size_t n = c->plane;
   uint16_t* st = reinterpret_cast<uint16_t*>(c->dStage.p);
-  unpackTexelF32Kernel<<<grid1(n), 256, 0, c->stream>>>(n, plane, st);
+  unpackTexelF32Kernel<<<grid1(n), 256, 0, c->stream>>>(n, (bias ? c->dProjBias.p : c->dProjColor.p) + (size_t)src * n, st);
   LAUNCHED("unpackTexelF32Kernel");
-  CU(cudaMemcpyAsync(bgr, st, n * 6, cudaMemcpyDefault, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return DERP_OK;
+  return copyPlanes(c, n * 6, {{bgr, st}});
 }
-
-int derp_get_proj_color(DerpCtx* c, int src, uint16_t* bgr) {
-  if (!bgr) return fail(DERP_EINVAL, "bad arguments");
-  int rc = checkProj(c, src, "derp_get_proj_color");
-  if (rc) return rc;
-  if ((rc = ensureTablesF32(c))) return rc;
-  return getTexels(c, c->dProjColor.p + (size_t)src * c->plane, bgr);
-}
-
-int derp_get_proj_bias(DerpCtx* c, int src, uint16_t* bgr) {
-  if (!bgr) return fail(DERP_EINVAL, "bad arguments");
-  int rc = checkProj(c, src, "derp_get_proj_bias");
-  if (rc) return rc;
-  if ((rc = ensureTablesF32(c))) return rc;
-  return getTexels(c, c->dProjBias.p + (size_t)src * c->plane, bgr);
-}
+int derp_get_proj_color(DerpCtx* c, int src, uint16_t* bgr) { return getTexels(c, src, bgr, "derp_get_proj_color", false); }
+int derp_get_proj_bias(DerpCtx* c, int src, uint16_t* bgr) { return getTexels(c, src, bgr, "derp_get_proj_bias", true); }
 
 int derp_get_counters(DerpCtx* c, uint64_t* cost_evals, uint64_t* src_hits) {
   if (!c) return fail(DERP_EINVAL, "null ctx");
@@ -1571,8 +1487,7 @@ int derp_debug_lower_bound(DerpCtx* c, int dst, int num_depths, float min_depth_
   int rc = checkDst(c, dst, "derp_debug_lower_bound", true);
   if (rc) return rc;
   if (num_depths < 2 || !stats) return fail(DERP_EINVAL, "derp_debug_lower_bound: bad arguments");
-  const int W = c->W, H = c->H;
-  const size_t n = c->plane;
+  // its own candidate table: the brute-force sweep's cached one in dDisparities stays as it is
   const std::vector<float> disparities = probeDisparities(num_depths, min_depth_m, max_depth_m);
   DevBuf<float> dTab;
   DevBuf<unsigned long long> dStats;
@@ -1580,32 +1495,16 @@ int derp_debug_lower_bound(DerpCtx* c, int dst, int num_depths, float min_depth_
   CU(dStats.ensure(5));
   CU(cudaMemsetAsync(dStats.p, 0, 5 * sizeof(unsigned long long), c->stream));
   if ((rc = ensureTablesF32(c))) return rc;
-  CU(c->dLb.ensure((size_t)num_depths * n));
-  CU(c->dSeed.ensure(n));
-  fillKernel<unsigned long long><<<grid1(n), 256, 0, c->stream>>>(n, c->dSeed.p, 0x7f7fffffffffffffull);
-  LAUNCHED("fillKernel");
   if ((rc = resetCounters(c))) return rc;
-  const LowerArgs la = lowerArgs(c, dst, dTab.p, num_depths, num_depths);
-  const int by = kBlockY;
-  SMEM_FITS(c->camSmem(), "lowerBoundCheckKernel");
-  c->k.sweepLower<<<dim3((W + kBlockX - 1) / kBlockX, (H + by - 1) / by, 1), dim3(kBlockX, by, 1), c->lowerSmem(), c->stream>>>(la);
-  LAUNCHED("sweepLowerKernel");
-  CheckArgs ca;
-  ca.v = la.v;
-  ca.fov = la.fov;
-  ca.fg = la.fg;
-  ca.bg = la.bg;
-  ca.disparities = dTab.p;
-  ca.D = num_depths;
-  ca.lb = c->dLb.p;
-  ca.stats = dStats.p;
-  c->k.lowerBoundCheck<<<grid2(W, H), block2(), c->camSmem(), c->stream>>>(ca);
+  if ((rc = checkSmem(c->camSmem(), "lowerBoundCheckKernel"))) return rc;
+  CU(c->dLb.ensure((size_t)num_depths * c->plane));
+  CU(c->dSeed.ensure(c->plane));
+  const DstArgs da = c->dstArgs(dst);  // after ensureTablesF32 (see dstArgs)
+  if ((rc = boundPass(c, da, dTab.p, num_depths, SweepShape{kBlockY, 1, num_depths}))) return rc;
+  const CheckArgs ca{da, dTab.p, num_depths, c->dLb.p, dStats.p};
+  c->k.lowerBoundCheck<<<grid2(c->W, c->H), block2(), c->camSmem(), c->stream>>>(ca);
   LAUNCHED("lowerBoundCheckKernel");
-  unsigned long long h[5];
-  CU(cudaMemcpyAsync(h, dStats.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  for (int i = 0; i < 5; ++i) stats[i] = h[i];
-  return DERP_OK;
+  return copyPlanes(c, 5 * sizeof(uint64_t), {{stats, dStats.p}});
 }
 
 // temporalJointBilateralFilter (TemporalBilateralFilter.h:126-215) for one camera

@@ -50,6 +50,14 @@ struct CostView {
   float one, b23;
 };
 
+// The per-destination block every cost kernel's arguments begin with (DerpCtx::dstArgs builds it on the host).
+struct DstArgs {
+  CostView v;
+  const uint8_t* fov;
+  const uint8_t* fg;  // nullable (all-pass)
+  const float* bg;    // nullable unless foreground masks are used
+};
+
 __device__ __forceinline__ int clampIdx(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
 
 // u16 -> float without the conversion pipe: 0x4B000000 | u is the float 2^23 + u exactly.

@@ -340,11 +340,7 @@ __global__ void fillKernel(size_t n, T* p, T v) {
 // minimum, then merges across chunks with a 64-bit atomicMin on (cost bits << 32 | index): for
 // non-negative floats the bit pattern is monotone, so the merge keeps the lowest cost and, among
 // equal costs, the lowest index — exactly the reference's first-strict-minimum scan.
-struct SweepArgs {
-  CostView v;
-  const uint8_t* fov;
-  const uint8_t* fg;       // nullable (all-pass)
-  const float* bg;         // nullable unless foreground masks are used
+struct SweepArgs : DstArgs {
   const float* disparities;  // [D] candidate table (probeDisparity)
   int D, chunk;
   unsigned long long* best;   // [H][W] packed
@@ -583,11 +579,7 @@ __global__ void activeScatterKernel(int W, int H, const int* __restrict__ prefix
 // exactly numProposals values for every processed pixel.  Whether a pixel is processed depends only
 // on masks and variance, so the draw index of pixel x is numProposals * (#processed pixels left of
 // x) = numProposals * prefix[x]: the row scan + LCG skip-ahead makes the row parallel and bit-identical.
-struct ProposalArgs {
-  CostView v;
-  const uint8_t* fov;
-  const uint8_t* fg;
-  const float* bg;
+struct ProposalArgs : DstArgs {
   const int* prefix;
   const int* list;       // active pixels
   const int* listCount;  // &rowOffset[H]
@@ -656,11 +648,7 @@ __global__ void __launch_bounds__(kPatchThreads, kPatchMinCtas) proposalKernel(c
 }
 
 // ---- K8: pingPongRectangle (Derp.cpp:403-478), one Jacobi iteration ------------------------------------
-struct PingPongArgs {
-  CostView v;
-  const uint8_t* fov;
-  const uint8_t* fg;
-  const float* bg;
+struct PingPongArgs : DstArgs {
   const float* disp;        // read
   const uint8_t* changed;   // read
   float* dispRes;           // write

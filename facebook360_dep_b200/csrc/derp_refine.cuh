@@ -21,11 +21,7 @@
 
 namespace derp {
 
-struct LowerArgs {
-  CostView v;
-  const uint8_t* fov;
-  const uint8_t* fg;   // nullable
-  const float* bg;     // nullable unless foreground masks are used
+struct LowerArgs : DstArgs {
   const float* disparities;
   int D, chunk;
   float* lb;                   // [D][H][W]
@@ -78,6 +74,9 @@ __global__ void __launch_bounds__(32 * kSweepMaxRows, kSweepMinCtas) sweepLowerK
   addCounters(a.counters, evals, hits);
 }
 
+// Not derived from DstArgs: its bg would take the parameter from 128 to 136 bytes, past the 128 bytes up to which nvcc
+// (12.9) loads a kernel parameter field by field instead of addressing it in parameter space.  That changes this
+// kernel's code and raises its spills (52 to 80 bytes with the 64-bit mask).
 struct SeedArgs {
   CostView v;
   const uint8_t* fov;
@@ -183,11 +182,7 @@ __global__ void __launch_bounds__(kPatchThreads, kPatchMinCtas) refineKernel(con
 // Validation of the bound itself (derp_debug_lower_bound): exact cost of EVERY (pixel, candidate) against lb.
 // stats: [0] evaluations compared, [1] violations (L > exact cost), [2] unknown (L == 0), [3] evaluations whose L is
 // within 5 % of the exact cost, [4] candidates that a per-pixel threshold at the true minimum would keep.
-struct CheckArgs {
-  CostView v;
-  const uint8_t* fov;
-  const uint8_t* fg;
-  const float* bg;
+struct CheckArgs : DstArgs {
   const float* disparities;
   int D;
   const float* lb;
