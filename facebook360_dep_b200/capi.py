@@ -728,12 +728,19 @@ _SWEEP_SIGS = {
     "derp_sweep_center_rig": (C.c_int, [_p(CameraDesc), C.c_int, C.c_int, _p(CameraDesc), C.c_void_p]),
     "derp_sweep_last_hits": (C.c_uint64, []),
     "derp_sweep_crop_width": (C.c_int, [C.c_uint64, C.c_void_p, _p(C.c_uint64)]),
+    "derp_project_equirect_masks": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, C.c_double, _p(C.c_void_p), C.c_void_p,
+                                              _p(C.c_void_p)]),
+    "derp_project_last_host_pixels": (C.c_uint64, []),
 }
 # derp_test_sweep_*_host: the same arguments as the entry point without the device
 _SWEEP_HOST_SIGS = {"derp_test_sweep_%s_host" % k: (C.c_int, _SWEEP_SIGS["derp_sweep_" + k][1][1:])
                     for k in ("overlaps", "equirect")}
 SWEEP_SYMBOLS = sorted(k for k in _SWEEP_SIGS if k.startswith("derp_sweep_"))
 SWEEP_TEST_HOOKS = sorted(_SWEEP_HOST_SIGS)
+_SWEEP_HOST_SIGS["derp_test_project_equirect_masks_host"] = (C.c_int,
+                                                            _SWEEP_SIGS["derp_project_equirect_masks"][1][1:])
+PROJECT_SYMBOLS = ["derp_project_equirect_masks", "derp_project_last_host_pixels",
+                   "derp_test_project_equirect_masks_host"]
 
 
 def rescaled_descs(descs, scale):
@@ -816,6 +823,32 @@ class SweepView(_Binding):
         else:
             self._check(self.lib.derp_sweep_equirect(device, *args))
         return outs
+
+    def project_masks(self, descs, masks, depth, device=0):
+        """ProjectEquirectsToCameras at `depth` m: masks[i] is camera i's equirect mask (uint8 [h, w], 0 / non-zero, or
+        a device pointer given as (ptr, w, h)); returns uint8 [int(res.y), int(res.x)] per camera, 0 or 255."""
+        ptrs, sizes, keep = [], [], []
+        for m in masks:
+            if isinstance(m, tuple):
+                ptrs.append(m[0])
+                sizes += [m[1], m[2]]
+            else:
+                m = np.ascontiguousarray(m, np.uint8)
+                keep.append(m)
+                ptrs.append(m.ctypes.data)
+                sizes += [m.shape[1], m.shape[0]]
+        sz = np.array(sizes, np.int32)
+        outs = [np.empty((int(d.resolution[1]), int(d.resolution[0])), np.uint8) for d in descs]
+        args = (descs, len(descs), float(depth), (C.c_void_p * len(ptrs))(*ptrs), sz.ctypes.data, _ptr_array(outs))
+        if self.host:
+            self._check(self.lib.derp_test_project_equirect_masks_host(*args))
+        else:
+            self._check(self.lib.derp_project_equirect_masks(device, *args))
+        return outs
+
+    def last_host_pixels(self):
+        """Pixels this thread's last project_masks call resolved on the host (the device could not prove them)."""
+        return int(self.lib.derp_project_last_host_pixels())
 
     def last_hits(self):
         """(sample, camera) pairs whose camera saw the point in this thread's last overlaps / equirect call."""

@@ -18,9 +18,17 @@ struct SweepScratch {
   DevBuf<int> widths, box;
   DevBuf<float4*> outs;
   DevBuf<unsigned long long> hits;
+  // derp_project_equirect_masks
+  DevBuf<uint8_t> maskUpload, maskOut;
+  DevBuf<derp::sweep::EqrMask> masks;
+  DevBuf<uint8_t*> maskOuts;
+  DevBuf<unsigned long long> undecided;
+  DevBuf<long long> resolved;
 };
 thread_local SweepScratch g_sweep;
 thread_local unsigned long long g_sweepHits = 0;  // contributing (sample, camera) pairs of the last call
+thread_local unsigned long long g_projectHostPixels = 0;  // pixels the last derp_project_equirect_masks left to the host
+constexpr unsigned long long kUndecidedCapacity = 1ull << 20;  // list entries kept between calls (grown on demand)
 
 // Cameras as the apps hold them (already rescaled), optionally centred on camera `center`
 int sweepCameras(const char* who, const DerpCameraDesc* cams, int n, int center, std::vector<DevCamera>& out) {
@@ -153,9 +161,130 @@ int uploadPlan(const EquirectPlan& p, const float* depths, int num, derp::sweep:
   return DERP_OK;
 }
 
+// Arguments of derp_project_equirect_masks and its host twin; W / H receive each camera's output size
+int checkProject(const char* who, const DerpCameraDesc* cams, int n, double depth, const uint8_t* const* masks,
+                 const int32_t* sizes, uint8_t* const* out, std::vector<DevCamera>& c, std::vector<int>& W,
+                 std::vector<int>& H) {
+  if (int rc = sweepCameras(who, cams, n, -1, c)) return rc;
+  if (!(depth > 0) || !std::isfinite(depth)) return fail(DERP_EINVAL, std::string(who) + ": depth must be > 0 and finite");
+  if (!masks || !sizes || !out) return fail(DERP_EINVAL, std::string(who) + ": masks, sizes and outputs are required");
+  W.resize(n);
+  H.resize(n);
+  for (int i = 0; i < n; ++i) {
+    if (!masks[i] || !out[i] || sizes[2 * i] < 1 || sizes[2 * i + 1] < 1 ||
+        (long long)sizes[2 * i] * sizes[2 * i + 1] >= (1ll << 31))
+      return fail(DERP_EINVAL, std::string(who) + ": bad mask or output " + std::to_string(i));
+    W[i] = (int)c[i].res[0];  // cv::Mat_<bool>(resolution.y(), resolution.x())
+    H[i] = (int)c[i].res[1];
+    if (W[i] < 1 || H[i] < 1 || (long long)W[i] * H[i] >= (1ll << 31))
+      return fail(DERP_EINVAL, std::string(who) + ": camera " + std::to_string(i) + " has no pixels or too many");
+  }
+  return DERP_OK;
+}
+
+// The host's decision at pixel (x, y) of camera c: the mask index, or -1 (the same DERP_HD code with the C library)
+long long projectPixelHost(const DevCamera& c, int x, int y, double depth, int mw, int mh) {
+  double w[3];
+  derp::sweep::rigPoint(c, x, y, depth, w);
+  return derp::sweep::eqrIndex(w[0], w[1], w[2], mw, mh);
+}
+
 }  // namespace
 
 extern "C" {
+
+int derp_project_equirect_masks(int device, const DerpCameraDesc* cams, int num_cams, double depth,
+                                const uint8_t* const* eqr_masks, const int32_t* mask_sizes, uint8_t* const* out) {
+  static const char* who = "derp_project_equirect_masks";
+  using derp::sweep::EqrMask;
+  std::vector<DevCamera> c;
+  std::vector<int> W, H;
+  if (int rc = checkProject(who, cams, num_cams, depth, eqr_masks, mask_sizes, out, c, W, H)) return rc;
+  CU(cudaSetDevice(device));
+  SweepScratch& s = g_sweep;
+  if (int rc = upload(s.cams, c.data(), num_cams)) return rc;
+  // masks: device-resident ones in place, the others uploaded into one scratch buffer
+  std::vector<EqrMask> m(num_cams);
+  std::vector<size_t> maskAt(num_cams, SIZE_MAX), outAt(num_cams, SIZE_MAX);
+  size_t maskTotal = 0, outTotal = 0;
+  int maxW = 0, maxH = 0;
+  for (int i = 0; i < num_cams; ++i) {
+    m[i] = EqrMask{eqr_masks[i], mask_sizes[2 * i], mask_sizes[2 * i + 1]};
+    if (!inPlace(eqr_masks[i], 1)) {
+      maskAt[i] = maskTotal;
+      maskTotal += (size_t)m[i].w * m[i].h;
+    }
+    if (!inPlace(out[i], 1)) {
+      outAt[i] = outTotal;
+      outTotal += (size_t)W[i] * H[i];
+    }
+    maxW = std::max(maxW, W[i]);
+    maxH = std::max(maxH, H[i]);
+  }
+  if (maskTotal) CU(s.maskUpload.ensure(maskTotal));
+  if (outTotal) CU(s.maskOut.ensure(outTotal));
+  std::vector<uint8_t*> outs(num_cams);
+  for (int i = 0; i < num_cams; ++i) {
+    if (maskAt[i] != SIZE_MAX) {
+      CU(cudaMemcpy(s.maskUpload.p + maskAt[i], eqr_masks[i], (size_t)m[i].w * m[i].h, cudaMemcpyDefault));
+      m[i].p = s.maskUpload.p + maskAt[i];
+    }
+    outs[i] = outAt[i] == SIZE_MAX ? out[i] : s.maskOut.p + outAt[i];
+  }
+  if (int rc = upload(s.masks, m.data(), num_cams)) return rc;
+  if (int rc = upload(s.maskOuts, outs.data(), num_cams)) return rc;
+  CU(s.hits.ensure(1));
+  CU(s.undecided.ensure(kUndecidedCapacity));
+  const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
+  const dim3 grid((maxW + block.x - 1) / block.x, (maxH + block.y - 1) / block.y, num_cams);
+  unsigned long long count = 0;
+  for (;;) {  // a second launch only when the undecided list overflowed (the kernel's decisions are deterministic)
+    CU(cudaMemset(s.hits.p, 0, sizeof(unsigned long long)));
+    derp::sweep::projectMasksKernel<<<grid, block>>>(s.cams.p, s.masks.p, depth, s.maskOuts.p, s.undecided.p,
+                                                     s.undecided.n, s.hits.p);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(&count, s.hits.p, sizeof count, cudaMemcpyDeviceToHost));
+    if (count <= s.undecided.n) break;
+    CU(s.undecided.ensure(count));
+  }
+  if (count) {
+    std::vector<unsigned long long> list(count);
+    CU(cudaMemcpy(list.data(), s.undecided.p, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    std::vector<long long> at(count);
+    for (size_t k = 0; k < count; ++k) {
+      const int i = (int)(list[k] >> 32);
+      const unsigned pixel = (unsigned)list[k];
+      at[k] = projectPixelHost(c[i], (int)(pixel % W[i]), (int)(pixel / W[i]), depth, m[i].w, m[i].h);
+    }
+    if (int rc = upload(s.resolved, at.data(), count)) return rc;
+    derp::sweep::resolveMasksKernel<<<(unsigned)((count + 255) / 256), 256>>>(s.masks.p, s.maskOuts.p, s.undecided.p,
+                                                                              s.resolved.p, (int)count);
+    CU(cudaGetLastError());
+  }
+  for (int i = 0; i < num_cams; ++i)
+    if (int rc = stageOut(out[i], outs[i], (size_t)W[i] * H[i])) return rc;
+  g_projectHostPixels = count;
+  return DERP_OK;
+}
+
+uint64_t derp_project_last_host_pixels(void) { return g_projectHostPixels; }
+
+int derp_test_project_equirect_masks_host(const DerpCameraDesc* cams, int num_cams, double depth,
+                                          const uint8_t* const* eqr_masks, const int32_t* mask_sizes,
+                                          uint8_t* const* out) {
+  std::vector<DevCamera> c;
+  std::vector<int> W, H;
+  if (int rc = checkProject("derp_test_project_equirect_masks_host", cams, num_cams, depth, eqr_masks, mask_sizes, out,
+                            c, W, H))
+    return rc;
+  for (int i = 0; i < num_cams; ++i)
+    for (int y = 0; y < H[i]; ++y)
+      for (int x = 0; x < W[i]; ++x) {
+        const long long at = projectPixelHost(c[i], x, y, depth, mask_sizes[2 * i], mask_sizes[2 * i + 1]);
+        out[i][(size_t)y * W[i] + x] = at >= 0 && eqr_masks[i][at] ? 255 : 0;
+      }
+  return DERP_OK;
+}
 
 int derp_sweep_overlaps(int device, const DerpCameraDesc* cams, int num_cams, const float* const* images_bgra,
                         const int32_t* image_sizes, int dst, const float* disparities, int num_slices, float* out) {

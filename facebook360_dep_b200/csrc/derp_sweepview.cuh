@@ -207,6 +207,213 @@ __global__ void __launch_bounds__(kSweepThreadsX * kSweepThreadsY) cropBoundsKer
 }
 #endif
 
+// ---- ProjectEquirectsToCameras (derp_project_equirect_masks) ------------------------------------------------
+// Per camera pixel (ProjectEquirectsToCameras.cpp:104-118): world = cam.rig({x + .5, y + .5}, depth) in fp64, then
+// worldToEquirect (ImageUtil.cpp:127-140) against the camera's W x H mask, the range test and mask(int(v H), int(u W)).
+// The reference's ImageUtil.cpp calls acos / atan2 with float arguments and resolves them to the float overloads
+// (acosf / atan2f; tests/test_eqr_project.py pins this against the compiled reference object).
+struct EqrMask {  // 16 bytes: one per camera
+  const uint8_t* p;
+  int w, h;
+};
+
+// The mask index int(v H) * W + int(u W) that the reference reads at rig point w, or -1 where it reads nothing: out of
+// range, or a NaN coordinate (z > 1 near a pole: the reference indexes the mask with int(NaN) there).
+DERP_HD long long eqrIndex(double wx, double wy, double wz, int W, int H) {
+  const float depth = (float)sqrt((wx * wx + wy * wy) + wz * wz);
+  const float x = (float)(wx / depth), y = (float)(wy / depth), z = (float)(wz / depth);
+  const float phi = acosf(z);
+  float theta = atan2f(y, x);
+  if (theta > 0) theta = (float)(theta - 2 * M_PI);
+  const float v = (float)(phi / M_PI);
+  const float u = (float)(-theta / (2.0f * M_PI));
+  const float px = u * (float)W, py = v * (float)H;
+  if (!(px >= 0 && py >= 0 && px < W && py < H)) return -1;
+  return (long long)(int)py * W + (int)px;
+}
+
+// rig({x + .5, y + .5}, depth) = position + ray * depth (Camera.h:141-143, ParametrizedLine::pointAt)
+DERP_HD void rigPoint(const DevCamera& c, int x, int y, double depth, double* w) {
+  double dir[3];
+  pixelRay(c, x + 0.5, y + 0.5, dir);
+  for (int k = 0; k < 3; ++k) w[k] = c.pos[k] + dir[k] * depth;
+}
+
+#if defined(__CUDACC__)
+// ---- the device's proof of a pixel ----
+// The device's acosf / atan2f / sin / cos / atan / asin are not glibc's to the last bit, so the device repeats the chain
+// on intervals and decides a pixel only when the interval fixes the theta > 0 branch, the range test and both truncated
+// indices; otherwise the host recomputes it.  Every IEEE operation of the chain is bracketed by its round-down and
+// round-up results (exact arithmetic lies between them, and round-to-nearest of any point of the operands' intervals
+// does too, the operations being monotone in each operand over the intervals where they are applied).  Each
+// transcendental result t is widened by (device bound + host bound + 1) ulp of |t|, the + 1 covering the difference
+// between the ulp at t and at the exact value, plus, for sin / cos, the width of their argument's interval (both are
+// 1-Lipschitz).  Device bounds: the CUDA C++ Programming Guide's maximum ulp errors (double sin, cos, atan, asin: 2;
+// acosf: 2; atan2f: 3).  Host bound: glibc's published maxima for x86_64 ("Known Maximum Errors in Math Functions")
+// are at most 1 ulp for these; 2 is budgeted.
+struct Iv {
+  double lo, hi;
+};
+constexpr double kTwoPi = 2 * M_PI;
+constexpr int kHostUlps = 2;
+constexpr int kSinUlps = 2 + kHostUlps + 1, kAtanUlps = 2 + kHostUlps + 1;  // double sin, cos, atan, asin
+constexpr int kAcosfUlps = 2 + kHostUlps + 1, kAtan2fUlps = 3 + kHostUlps + 1;
+
+// extra + k ulp of a double function's result t, rounded up (ulp(t) <= 2^-52 |t|; 2^-1074 below the normal range)
+__device__ __forceinline__ double errD(double t, int k, double extra) {
+  return __dadd_ru(__dmul_ru(k * 0x1p-52, __dadd_ru(fabs(t), extra)), __dadd_ru(extra, k * 0x1p-1074));
+}
+__device__ __forceinline__ Iv widenD(double t, int k, double extra) {
+  const double e = errD(t, k, extra);
+  return Iv{__dadd_rd(t, -e), __dadd_ru(t, e)};
+}
+// the same for a float function, in double (ulp(t) <= 2^-23 |t|; 2^-149 below the normal range)
+__device__ __forceinline__ Iv widenF(float t, int k) {
+  const double e = __dadd_ru(__dmul_ru(k * 0x1p-23, fabs((double)t)), k * 0x1p-149);
+  return Iv{__dadd_rd(t, -e), __dadd_ru(t, e)};
+}
+__device__ __forceinline__ Iv ivAdd(Iv a, Iv b) { return Iv{__dadd_rd(a.lo, b.lo), __dadd_ru(a.hi, b.hi)}; }
+__device__ __forceinline__ Iv ivScale(Iv a, double s) {  // a * s, s a point
+  return s >= 0 ? Iv{__dmul_rd(a.lo, s), __dmul_ru(a.hi, s)} : Iv{__dmul_rd(a.hi, s), __dmul_ru(a.lo, s)};
+}
+__device__ __forceinline__ Iv ivDivPos(Iv a, double d) { return Iv{__ddiv_rd(a.lo, d), __ddiv_ru(a.hi, d)}; }  // d > 0
+__device__ __forceinline__ Iv ivSqr(Iv a) {
+  if (a.lo >= 0) return Iv{__dmul_rd(a.lo, a.lo), __dmul_ru(a.hi, a.hi)};
+  if (a.hi <= 0) return Iv{__dmul_rd(a.hi, a.hi), __dmul_ru(a.lo, a.lo)};
+  return Iv{0.0, fmax(__dmul_ru(a.lo, a.lo), __dmul_ru(a.hi, a.hi))};
+}
+// a / d with d a positive interval
+__device__ __forceinline__ Iv ivDiv(Iv a, Iv d) {
+  return Iv{fmin(__ddiv_rd(a.lo, d.lo), __ddiv_rd(a.lo, d.hi)), fmax(__ddiv_ru(a.hi, d.lo), __ddiv_ru(a.hi, d.hi))};
+}
+__device__ __forceinline__ Iv ivFloat(Iv a) { return Iv{__double2float_rd(a.lo), __double2float_ru(a.hi)}; }
+
+// rigPoint on intervals: sensorToCamera's branches depend only on exactly computed values (the sensor point, its norm
+// and undistort's result), so the interval follows the same branch as any IEEE evaluation
+__device__ __forceinline__ void rigPointIv(const DevCamera& c, int px, int py, double depth, Iv* w) {
+  const double sx = (px + 0.5 - c.principal[0]) / c.focal[0];
+  const double sy = (py + 0.5 - c.principal[1]) / c.focal[1];
+  const double squaredNorm = sx * sx + sy * sy;
+  Iv u[3];
+  if (squaredNorm == 0) {
+    u[0] = u[1] = Iv{0.0, 0.0};
+    u[2] = Iv{-1.0, -1.0};
+  } else {
+    const double norm = sqrt(squaredNorm);
+    const double r = undistort(c, norm);
+    double theta, eTheta = 0;  // theta +- eTheta holds the host's theta
+    if (c.type == DERP_CAM_FTHETA) {
+      theta = r;
+    } else if (c.type == DERP_CAM_RECTILINEAR) {
+      theta = atan(r);
+      eTheta = errD(theta, kAtanUlps, 0);
+    } else if (c.type == DERP_CAM_EQUISOLID) {
+      if (r <= 2) {
+        const double a = asin(r / 2);
+        theta = 2 * a;
+        eTheta = 2 * errD(a, kAtanUlps, 0);
+      } else {
+        theta = 3.14159265358979323846;
+      }
+    } else {
+      if (r <= 1) {
+        theta = asin(r);
+        eTheta = errD(theta, kAtanUlps, 0);
+      } else {
+        theta = 3.14159265358979323846 / 2;
+      }
+    }
+    const Iv s = widenD(sin(theta), kSinUlps, eTheta), co = widenD(cos(theta), kSinUlps, eTheta);
+    const Iv f = ivDivPos(s, norm);
+    u[0] = ivScale(f, sx);
+    u[1] = ivScale(f, sy);
+    u[2] = Iv{-co.hi, -co.lo};
+  }
+  for (int k = 0; k < 3; ++k) {
+    const Iv d = ivAdd(ivAdd(ivScale(u[0], c.rot[k]), ivScale(u[1], c.rot[3 + k])), ivScale(u[2], c.rot[6 + k]));
+    w[k] = ivAdd(Iv{c.pos[k], c.pos[k]}, ivScale(d, depth));
+  }
+}
+
+// p < 0 -> -1, p >= n -> n, else int(p): monotone in p, so equal codes at both ends fix the whole interval
+__device__ __forceinline__ int rangeCode(float p, int n) { return p < 0 ? -1 : p >= n ? n : (int)p; }
+
+// eqrIndex on the interval w: the index (>= 0) or -1 when proven, -2 when the interval does not decide
+__device__ __forceinline__ long long eqrIndexProven(const Iv* w, int W, int H) {
+  constexpr long long kUndecided = -2;
+  const Iv n = ivAdd(ivAdd(ivSqr(w[0]), ivSqr(w[1])), ivSqr(w[2]));
+  const Iv depth = ivFloat(Iv{__dsqrt_rd(n.lo), __dsqrt_ru(n.hi)});
+  if (!(depth.lo > 0)) return kUndecided;
+  const Iv x = ivFloat(ivDiv(w[0], depth)), y = ivFloat(ivDiv(w[1], depth)), z = ivFloat(ivDiv(w[2], depth));
+  if (z.lo > 1 || z.hi < -1) return -1;                     // acos is NaN at every point: the pixel stays 0
+  if (!(z.hi <= 1 && z.lo >= -1)) return kUndecided;        // NaN at some points only
+  const Iv phi = Iv{widenF(acosf((float)z.hi), kAcosfUlps).lo, widenF(acosf((float)z.lo), kAcosfUlps).hi};
+  // atan2 over the box x * y: off the origin and the branch cut (x < 0, y = 0) its extremes are at the corners
+  if (x.lo <= 0 && x.hi >= 0 && y.lo <= 0 && y.hi >= 0) return kUndecided;
+  if (x.lo < 0 && y.lo <= 0 && y.hi >= 0) return kUndecided;
+  double tlo = INFINITY, thi = -INFINITY;
+  for (int k = 0; k < 4; ++k) {
+    const Iv t = widenF(atan2f((float)((k & 1) ? y.hi : y.lo), (float)((k & 2) ? x.hi : x.lo)), kAtan2fUlps);
+    tlo = fmin(tlo, t.lo);
+    thi = fmax(thi, t.hi);
+  }
+  Iv theta = ivFloat(Iv{tlo, thi});  // the host's theta is a float inside the widened range
+  if (theta.lo > 0) {
+    theta = ivFloat(Iv{__dadd_rd(theta.lo, -kTwoPi), __dadd_ru(theta.hi, -kTwoPi)});
+  } else if (theta.hi > 0) {
+    return kUndecided;
+  }
+  const Iv v = ivFloat(ivDivPos(ivFloat(phi), M_PI));
+  const Iv u = ivFloat(ivDivPos(Iv{-theta.hi, -theta.lo}, kTwoPi));
+  const float fW = (float)W, fH = (float)H;
+  const float pxl = __fmul_rd((float)u.lo, fW), pxh = __fmul_ru((float)u.hi, fW);
+  const float pyl = __fmul_rd((float)v.lo, fH), pyh = __fmul_ru((float)v.hi, fH);
+  if (!(pxl <= pxh) || !(pyl <= pyh)) return kUndecided;  // NaN
+  const int xl = rangeCode(pxl, W), xh = rangeCode(pxh, W), yl = rangeCode(pyl, H), yh = rangeCode(pyh, H);
+  if ((xl == xh && (xl < 0 || xl >= W)) || (yl == yh && (yl < 0 || yl >= H))) return -1;  // skipped either way
+  if (xl != xh || yl != yh) return kUndecided;
+  return (long long)yl * W + xl;
+}
+
+// One thread per pixel of camera blockIdx.z: out = 255 where the proven mask texel is set, 0 where it is not or where
+// the reference skips the pixel; undecided pixels are written 1 and listed (camera << 32 | pixel) for the host
+__global__ void __launch_bounds__(kSweepThreadsX * kSweepThreadsY) projectMasksKernel(
+    const DevCamera* __restrict__ gCams, const EqrMask* __restrict__ masks, double depth, uint8_t* const* outs,
+    unsigned long long* __restrict__ undecided, unsigned long long capacity, unsigned long long* __restrict__ count) {
+  __shared__ DevCamera cam;
+  const int i = blockIdx.z;
+  if (threadIdx.x == 0 && threadIdx.y == 0) cam = gCams[i];
+  __syncthreads();
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const int W = (int)cam.res[0], H = (int)cam.res[1];
+  if (x >= W || y >= H) return;
+  const EqrMask m = masks[i];
+  Iv w[3];
+  rigPointIv(cam, x, y, depth, w);
+  const long long at = eqrIndexProven(w, m.w, m.h);
+  uint8_t v = 0;
+  if (at >= 0) {
+    v = m.p[at] ? 255 : 0;
+  } else if (at == -2) {
+    v = 1;
+    const unsigned long long slot = atomicAdd(count, 1ull);
+    if (slot < capacity) undecided[slot] = (unsigned long long)i << 32 | (unsigned)(y * W + x);
+  }
+  outs[i][(size_t)y * W + x] = v;
+}
+
+// Writes the host's decisions: at[k] is the mask index of undecided pixel list[k], or -1
+__global__ void resolveMasksKernel(const EqrMask* __restrict__ masks, uint8_t* const* outs,
+                                   const unsigned long long* __restrict__ list, const long long* __restrict__ at,
+                                   int num) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= num) return;
+  const int i = (int)(list[k] >> 32);
+  const unsigned pixel = (unsigned)list[k];
+  outs[i][pixel] = at[k] >= 0 && masks[i].p[at[k]] ? 255 : 0;
+}
+#endif
+
 // ---- host side ----------------------------------------------------------------------------------------------
 namespace host {
 

@@ -601,7 +601,7 @@ inline void writeExrFloatChannels(const fs::path& path, const float* data, int w
 }
 inline void writeExrFloat(const fs::path& path, const float* data, int w, int h) { writeExrFloatChannels(path, data, w, h, 1); }
 
-// 16-bit PNG, `channels` = 1 (gray) or 3 (BGR input, written as RGB)
+// 16-bit PNG, `channels` = 1 (gray), 3 (BGR input, written as RGB) or 4 (BGRA input, written as RGBA)
 inline void writePng16(const fs::path& path, const uint16_t* data, int w, int h, int channels) {
   std::ofstream f(path, std::ios::binary);
   CHECK(f.good()) << "failed to save image: " << path.string();
@@ -611,7 +611,7 @@ inline void writePng16(const fs::path& path, const uint16_t* data, int w, int h,
   ihdr[0] = w >> 24; ihdr[1] = w >> 16; ihdr[2] = w >> 8; ihdr[3] = w;
   ihdr[4] = h >> 24; ihdr[5] = h >> 16; ihdr[6] = h >> 8; ihdr[7] = h;
   ihdr[8] = 16;
-  ihdr[9] = channels == 1 ? 0 : 2;
+  ihdr[9] = channels == 1 ? 0 : channels == 4 ? 6 : 2;  // grey, RGB from BGR, RGBA from BGRA
   pngChunk(f, "IHDR", ihdr);
   const size_t stride = (size_t)w * channels * 2;
   std::vector<uint8_t> raw((stride + 1) * h);
@@ -620,7 +620,7 @@ inline void writePng16(const fs::path& path, const uint16_t* data, int w, int h,
     *out++ = 0;
     for (int x = 0; x < w; ++x)
       for (int c = 0; c < channels; ++c) {
-        const int sc = channels == 3 ? 2 - c : c;
+        const int sc = channels >= 3 && c < 3 ? 2 - c : c;
         const uint16_t v = data[((size_t)y * w + x) * channels + sc];
         *out++ = (uint8_t)(v >> 8);
         *out++ = (uint8_t)v;

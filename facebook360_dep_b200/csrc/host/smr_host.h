@@ -99,19 +99,19 @@ inline void backgroundEquirect(float* fore, int width, int height, const float* 
     }
 }
 
-// cv_util::convertImage<cv::Vec3w> of a Vec4f image: convertTo(CV_16U, 65535) (saturate_cast of cvRound(v * 65535):
-// round half to even, NaN -> 0) and BGRA -> BGR
-inline std::vector<uint16_t> toPng16(const float* bgra, size_t n) {
-  std::vector<uint16_t> out(n * 3);
+// cv_util::convertImage<cv::Vec3w> (channels = 3) or <cv::Vec4w> (channels = 4) of a Vec4f image: convertTo(CV_16U,
+// 65535) (saturate_cast of cvRound(v * 65535): round half to even, NaN -> 0), with BGRA -> BGR for 3 channels
+inline std::vector<uint16_t> toPng16(const float* bgra, size_t n, int channels = 3) {
+  std::vector<uint16_t> out(n * channels);
   for (size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 3; ++c) {
+    for (int c = 0; c < channels; ++c) {
       const float v = bgra[4 * i + c] * 65535.0f;
       uint16_t u = 0;
       if (v > -2147483648.0f && v < 2147483648.0f) {
         const long r = std::lrintf(v);
         u = (uint16_t)(r < 0 ? 0 : r > 65535 ? 65535 : r);
       }
-      out[3 * i + c] = u;
+      out[channels * i + c] = u;
     }
   return out;
 }

@@ -1,6 +1,7 @@
 /*
  * derp_sweepview.h — C ABI of the constant-depth sweep slices of GenerateCameraOverlaps
- * (source/render/GenerateCameraOverlaps.cpp) and GenerateEquirect (source/render/GenerateEquirect.cpp) on the H100.
+ * (source/render/GenerateCameraOverlaps.cpp) and GenerateEquirect (source/render/GenerateEquirect.cpp), and of the
+ * constant-depth equirect mask projection of ProjectEquirectsToCameras (source/conversion), on the H100.
  *
  * Exported by facebook360_dep_b200/libderp_b200.so next to the depth ABI of derp_b200.h, whose conventions it follows:
  * 0 on success, a negative DERP_E* code on failure with the message in derp_last_error(); images row-major, top row
@@ -40,6 +41,20 @@
  *
  * derp_test_sweep_overlaps_host / derp_test_sweep_equirect_host: the same per-pixel functions (DERP_HD), run on the host
  * with host pointers, for tests without a GPU.
+ *
+ * derp_project_equirect_masks: ProjectEquirectsToCameras' projection (ProjectEquirectsToCameras.cpp:94-125) of one
+ * frame for the whole rig.  eqr_masks[i] is camera i's equirect mask, bytes 0 / non-zero, of mask_sizes[2 i] x
+ * mask_sizes[2 i + 1] pixels (width, height; any size per camera); out[i] receives [int(res.y)][int(res.x)] bytes, 255
+ * where the reference sets the camera mask and 0 elsewhere.  Per pixel: world = rig({x + .5, y + .5}, depth) in fp64,
+ * worldToEquirect (ImageUtil.cpp:127-140, float acosf / atan2f), the range test and mask(int(v H), int(u W)).  A NaN
+ * equirect coordinate (near a pole, where float(norm) < |z| makes acos NaN and the reference indexes the mask with
+ * int(NaN)) leaves the pixel 0; no mask byte outside the image is read for any input.  The device decides a pixel only
+ * when an interval evaluation of the chain proves the reference's decision; the other pixels are recomputed on the
+ * host with the same code and the C library (derp_sweepview.cuh documents the bound).
+ * derp_project_last_host_pixels: the number of pixels the calling thread's last derp_project_equirect_masks resolved on
+ * the host.
+ * derp_test_project_equirect_masks_host: the same per-pixel function on the host, with host pointers, for tests without a
+ * GPU.
  */
 #ifndef DERP_SWEEPVIEW_H_
 #define DERP_SWEEPVIEW_H_
@@ -68,6 +83,13 @@ int derp_test_sweep_equirect_host(const DerpCameraDesc* cams, int num_cams, int 
                                   const float* const* images_bgra, const int32_t* image_sizes, uint64_t height,
                                   const float* depths, int num_depths, const double* bounds, int black_bg,
                                   float* const* out);
+
+int derp_project_equirect_masks(int device, const DerpCameraDesc* cams, int num_cams, double depth,
+                                const uint8_t* const* eqr_masks, const int32_t* mask_sizes, uint8_t* const* out);
+uint64_t derp_project_last_host_pixels(void);
+int derp_test_project_equirect_masks_host(const DerpCameraDesc* cams, int num_cams, double depth,
+                                          const uint8_t* const* eqr_masks, const int32_t* mask_sizes,
+                                          uint8_t* const* out);
 
 #ifdef __cplusplus
 }
