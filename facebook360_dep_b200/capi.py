@@ -906,3 +906,146 @@ class EqrMesh(_Binding):
         else:
             self._check(self.lib.derp_equirect_mesh(*head, *tail))
         return vtx[:nv.value].copy(), idx[:nf.value].copy()
+
+
+# ---- include/derp_rigsim.h ----------------------------------------------------------------------------------------
+RIGSIM_SCENES = {"icosahedron": 0, "cube": 1, "ground_plane": 2}
+
+
+class RigsimSceneParams(C.Structure):
+    _fields_ = [("scene", C.c_int32), ("num_random_icosahedrons", C.c_int32), ("red_triangle", C.c_int32),
+                ("reserved", C.c_int32), ("min_icosahedron_dist", C.c_double), ("max_icosahedron_dist", C.c_double),
+                ("min_icosahedron_radius", C.c_double), ("max_icosahedron_radius", C.c_double),
+                ("ground_plane_dist_m", C.c_double)]
+
+
+class RigsimRender(C.Structure):
+    _fields_ = [("anti_alias_supersample", C.c_int32), ("marble", C.c_int32), ("marble_scale", C.c_double),
+                ("interpupillary_radius", C.c_double), ("skybox_bgr", C.c_void_p), ("skybox_width", C.c_int32),
+                ("skybox_height", C.c_int32), ("ceiling_bgr", C.c_void_p), ("ceiling_cols", C.c_int32),
+                ("ceiling_rows", C.c_int32), ("ceiling_position", C.c_double), ("ceiling_width", C.c_double),
+                ("ceiling_depth", C.c_double)]
+
+
+RIGSIM_TRIANGLE = np.dtype([(k, np.float32, (3,)) for k in ("v0", "v1", "v2", "e1", "e2", "normal", "color")])
+RIGSIM_NODE = np.dtype([("center", np.float32, (3,)), ("radius", np.float32), ("first", np.int32),
+                        ("count", np.int32), ("escape", np.int32), ("reserved", np.int32)])
+
+_RIGSIM_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_rigsim_scene_create": (C.c_int, [_p(RigsimSceneParams), _p(C.c_void_p)]),
+    "derp_rigsim_scene_destroy": (None, [C.c_void_p]),
+    "derp_rigsim_scene_info": (C.c_int, [C.c_void_p, _p(C.c_int32), _p(C.c_int32), _p(C.c_int32)]),
+    "derp_rigsim_scene_get": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "derp_rigsim_render_cameras": (C.c_int, [C.c_int, C.c_void_p, _p(RigsimRender), _p(CameraDesc), C.c_int,
+                                             _p(C.c_void_p), _p(C.c_void_p)]),
+    "derp_rigsim_render_equirect": (C.c_int, [C.c_int, C.c_void_p, _p(RigsimRender), C.c_int, C.c_int, C.c_int,
+                                              C.c_void_p, C.c_void_p]),
+    "derp_rigsim_last_host_rays": (C.c_uint64, []),
+    "derp_rigsim_last_rays": (C.c_uint64, []),
+    "derp_rigsim_trace_host": (C.c_int, [C.c_void_p, _p(RigsimRender), C.c_void_p, C.c_int, C.c_void_p]),
+    "derp_test_rigsim_area": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+}
+RIGSIM_SYMBOLS = sorted(k for k in _RIGSIM_SIGS if k.startswith("derp_rigsim_"))
+
+
+class RigSim(_Binding):
+    """ctypes binding of include/derp_rigsim.h on a loaded library: ``RigSim(load_cuda())``.
+
+    ``scene(...)`` builds the scene and its BVH on the host from the process's rand() stream (seed it with
+    ``srand``); the render calls take the scene handle, an 8-bit BGR skybox and RigSimulator's rendering flags."""
+
+    def __init__(self, library):
+        self.path, self.lib = _bind(library, _RIGSIM_SIGS)
+        self.libc = C.CDLL(None)
+        self.libc.rand.restype = C.c_int
+
+    def srand(self, seed):
+        """Seeds the C library's rand(), which the scene and the BVH consume (the same stream the process shares)."""
+        self.libc.srand(C.c_uint(seed))
+
+    def rand(self):
+        """The next rand() value (tests compare the stream position a scene build leaves)."""
+        return int(self.libc.rand())
+
+    def scene(self, scene="icosahedron", num_random_icosahedrons=250, min_icosahedron_dist=100.0,
+              max_icosahedron_dist=250.0, min_icosahedron_radius=20.0, max_icosahedron_radius=50.0,
+              red_triangle=False, ground_plane_dist_m=1.70):
+        p = RigsimSceneParams(RIGSIM_SCENES[scene], num_random_icosahedrons, int(bool(red_triangle)), 0,
+                              min_icosahedron_dist, max_icosahedron_dist, min_icosahedron_radius,
+                              max_icosahedron_radius, ground_plane_dist_m)
+        h = C.c_void_p()
+        self._check(self.lib.derp_rigsim_scene_create(C.byref(p), C.byref(h)))
+        return h
+
+    def destroy(self, scene):
+        self.lib.derp_rigsim_scene_destroy(scene)
+
+    def scene_arrays(self, scene):
+        """(triangles RIGSIM_TRIANGLE [nt], nodes RIGSIM_NODE [nn], leaf triangle indices int32 [nl]), BVH in preorder."""
+        nt, nn, nl = C.c_int32(), C.c_int32(), C.c_int32()
+        self._check(self.lib.derp_rigsim_scene_info(scene, C.byref(nt), C.byref(nn), C.byref(nl)))
+        tris = np.zeros(max(nt.value, 1), RIGSIM_TRIANGLE)
+        nodes = np.zeros(nn.value, RIGSIM_NODE)
+        leaf = np.zeros(max(nl.value, 1), np.int32)
+        self._check(self.lib.derp_rigsim_scene_get(scene, tris.ctypes.data, nodes.ctypes.data, leaf.ctypes.data))
+        return tris[:nt.value], nodes, leaf[:nl.value]
+
+    @staticmethod
+    def render_opts(skybox, aas=1, marble=False, marble_scale=0.1, interpupillary_radius=3.2, ceiling=None,
+                    ceiling_position=0.0, ceiling_width=0.0, ceiling_depth=0.0):
+        """The rendering flags as a RigsimRender; skybox / ceiling are uint8 [h, w, 3] BGR arrays (kept alive by the
+        returned tuple's second element)."""
+        sky = np.ascontiguousarray(skybox, np.uint8)
+        ceil = None if ceiling is None else np.ascontiguousarray(ceiling, np.uint8)
+        o = RigsimRender(int(aas), int(bool(marble)), marble_scale, interpupillary_radius, sky.ctypes.data,
+                         sky.shape[1], sky.shape[0], None if ceil is None else ceil.ctypes.data,
+                         0 if ceil is None else ceil.shape[1], 0 if ceil is None else ceil.shape[0],
+                         ceiling_position, ceiling_width, ceiling_depth)
+        return o, (sky, ceil)
+
+    def render_cameras(self, scene, descs, skybox, outs=None, device=0, **opts):
+        """renderCamera for every camera (no noise): a list of (bgr float32 [h, w, 3] = 255 * B, G, R, depth float32
+        [h, w]).  ``outs``: optional (bgr pointers, depth pointers) of device memory written in place."""
+        o, keep = self.render_opts(skybox, **opts)
+        if isinstance(descs, (list, tuple)):
+            descs = (CameraDesc * len(descs))(*descs)
+        if outs is None:
+            res = [(np.empty((int(d.resolution[1]), int(d.resolution[0]), 3), np.float32),
+                    np.empty((int(d.resolution[1]), int(d.resolution[0])), np.float32)) for d in descs]
+            b, dp = _ptr_array([r[0] for r in res]), _ptr_array([r[1] for r in res])
+        else:
+            res = None
+            b, dp = (C.c_void_p * len(descs))(*outs[0]), (C.c_void_p * len(descs))(*outs[1])
+        self._check(self.lib.derp_rigsim_render_cameras(device, scene, C.byref(o), descs, len(descs), b, dp))
+        return res
+
+    def render_equirect(self, scene, width, height, skybox, stereo=False, device=0, **opts):
+        """renderMonoEquirect: (bgr [h, w, 3], clamp(1 / depth) [h, w]); stereo: (left bgr, right bgr)."""
+        o, keep = self.render_opts(skybox, **opts)
+        out0 = np.empty((height, width, 3), np.float32)
+        out1 = np.empty((height, width, 3) if stereo else (height, width), np.float32)
+        self._check(self.lib.derp_rigsim_render_equirect(device, scene, C.byref(o), int(bool(stereo)), width, height,
+                                                         out0.ctypes.data, out1.ctypes.data))
+        return out0, out1
+
+    def area(self, src, k, device=0):
+        """The render's INTER_AREA by the integer factor k on the GPU (derp_test_rigsim_area): float [h / k, w / k(, cn)]."""
+        s = np.ascontiguousarray(src, np.float32)
+        cn = 1 if s.ndim == 2 else s.shape[2]
+        out = np.empty((s.shape[0] // k, s.shape[1] // k) + s.shape[2:], np.float32)
+        self._check(self.lib.derp_test_rigsim_area(device, s.ctypes.data, out.shape[1], out.shape[0], cn, k,
+                                                   out.ctypes.data))
+        return out
+
+    def last_host_rays(self):
+        """(rays whose sky texel the host resolved, supersample rays traced) in this thread's last render."""
+        return int(self.lib.derp_rigsim_last_host_rays()), int(self.lib.derp_rigsim_last_rays())
+
+    def trace_host(self, scene, rays, skybox, **opts):
+        """traceRayToGetColor on the host for float32 rays [n, 6] (origin, direction): float32 [n, 4] = B, G, R, depth."""
+        o, keep = self.render_opts(skybox, **opts)
+        r = np.ascontiguousarray(rays, np.float32).reshape(-1, 6)
+        out = np.empty((len(r), 4), np.float32)
+        self._check(self.lib.derp_rigsim_trace_host(scene, C.byref(o), r.ctypes.data, len(r), out.ctypes.data))
+        return out
