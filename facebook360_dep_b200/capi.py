@@ -1049,3 +1049,102 @@ class RigSim(_Binding):
         out = np.empty((len(r), 4), np.float32)
         self._check(self.lib.derp_rigsim_trace_host(scene, C.byref(o), r.ctypes.data, len(r), out.ctypes.data))
         return out
+
+
+# ---- include/derp_riganalysis.h -----------------------------------------------------------------------------------
+_RIGANALYSIS_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_rig_coverage": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                    C.c_int, C.c_void_p]),
+    "derp_rig_equirect_coverage": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                             C.c_double, C.c_void_p, C.c_void_p]),
+    "derp_rig_camera_coverage": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_double,
+                                           C.c_void_p]),
+    "derp_rig_cross_section": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "derp_rig_analysis_last_host_points": (C.c_uint64, []),
+    "derp_test_rig_coverage_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                              C.c_int, C.c_void_p]),
+    "derp_test_rig_equirect_coverage_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                       C.c_double, C.c_void_p, C.c_void_p]),
+    "derp_test_rig_camera_coverage_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_double,
+                                                     C.c_void_p]),
+    "derp_test_rig_cross_section_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+}
+RIGANALYSIS_SYMBOLS = sorted(k for k in _RIGANALYSIS_SIGS if k.startswith("derp_rig_"))
+
+
+class RigAnalysis(_Binding):
+    """ctypes binding of include/derp_riganalysis.h on a loaded library: ``RigAnalysis(load_cuda())``.
+
+    Every call takes the rig as CameraDesc entries (a list or a ctypes array) and, optionally, ``rot``: float64
+    [n, 3, 3] rotation matrices (rows right, up, backward) used as given.  ``host=True`` runs the host per-point code
+    (derp_test_rig_*_host) instead of the GPU.  ``out`` (where taken) is a device pointer written in place."""
+
+    def __init__(self, library):
+        self.path, self.lib = _bind(library, _RIGANALYSIS_SIGS)
+
+    @staticmethod
+    def _rig(descs, rot):
+        if isinstance(descs, (list, tuple)):
+            descs = (CameraDesc * len(descs))(*descs)
+        r = None if rot is None else np.ascontiguousarray(rot, np.float64).reshape(len(descs), 9)
+        return descs, r, (None if r is None else r.ctypes.data)
+
+    def coverage(self, descs, samples, distances, rot=None, host=False, device=0):
+        """uint64 [len(distances), n + 1]: per distance, the number of samples seen by exactly k cameras."""
+        descs, keep, r = self._rig(descs, rot)
+        s = np.ascontiguousarray(samples, np.float64).reshape(-1, 3)
+        d = np.ascontiguousarray(distances, np.float64)
+        hist = np.zeros((len(d), len(descs) + 1), np.uint64)
+        if host:
+            self._check(self.lib.derp_test_rig_coverage_host(descs, r, len(descs), s.ctypes.data, len(s),
+                                                             d.ctypes.data, len(d), hist.ctypes.data))
+        else:
+            self._check(self.lib.derp_rig_coverage(device, descs, r, len(descs), s.ctypes.data, len(s), d.ctypes.data,
+                                                   len(d), hist.ctypes.data))
+        return hist
+
+    def equirect(self, descs, width, height, distance, rot=None, host=False, device=0, out=None):
+        """(counts int32 [height, width], minTimingDiff float32 [height, width]); with ``out`` = (counts, timing)
+        device pointers they are written in place and (None, None) is returned."""
+        descs, keep, r = self._rig(descs, rot)
+        if out is None:
+            counts, timing = np.empty((height, width), np.int32), np.empty((height, width), np.float32)
+            pc, pt = counts.ctypes.data, timing.ctypes.data
+        else:
+            counts = timing = None
+            pc, pt = out
+        if host:
+            self._check(self.lib.derp_test_rig_equirect_coverage_host(descs, r, len(descs), width, height, distance,
+                                                                      pc, pt))
+        else:
+            self._check(self.lib.derp_rig_equirect_coverage(device, descs, r, len(descs), width, height, distance,
+                                                            pc, pt))
+        return counts, timing
+
+    def camera(self, descs, cam, distance, rot=None, host=False, device=0, out=None):
+        """int32 [int(res.y), int(res.x)] of camera ``cam``."""
+        descs, keep, r = self._rig(descs, rot)
+        d = descs[cam]
+        counts = None if out is not None else np.empty((int(d.resolution[1]), int(d.resolution[0])), np.int32)
+        p = out if out is not None else counts.ctypes.data
+        if host:
+            self._check(self.lib.derp_test_rig_camera_coverage_host(descs, r, len(descs), cam, distance, p))
+        else:
+            self._check(self.lib.derp_rig_camera_coverage(device, descs, r, len(descs), cam, distance, p))
+        return counts
+
+    def cross_section(self, descs, dim=400, rot=None, host=False, device=0, out=None):
+        """int32 [dim, dim]."""
+        descs, keep, r = self._rig(descs, rot)
+        counts = None if out is not None else np.empty((dim, dim), np.int32)
+        p = out if out is not None else counts.ctypes.data
+        if host:
+            self._check(self.lib.derp_test_rig_cross_section_host(descs, r, len(descs), dim, p))
+        else:
+            self._check(self.lib.derp_rig_cross_section(device, descs, r, len(descs), dim, p))
+        return counts
+
+    def last_host_points(self):
+        """The points this thread's last GPU call resolved on the host."""
+        return int(self.lib.derp_rig_analysis_last_host_points())

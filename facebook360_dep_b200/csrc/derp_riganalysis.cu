@@ -1,0 +1,400 @@
+// include/derp_riganalysis.h: RigAnalyzer's coverage counts on sm_90a (per-point code and proof in
+// derp_riganalysis.cuh), the host resolution of the points the device leaves undecided, and the host instantiation of
+// the per-point code for the CPU tests.
+#include "derp_host.cuh"
+#include "derp_riganalysis.cuh"
+#include "../../include/derp_riganalysis.h"
+
+using namespace derp;
+using namespace derp::rig;
+
+namespace {
+
+struct RigScratch {
+  DevBuf<DevCamera> cams;
+  DevBuf<double> tabs;
+  DevBuf<unsigned long long> hist, undecided, count;
+  DevBuf<int32_t> counts, resolvedCounts;
+  DevBuf<float> timing, resolvedTiming;
+};
+thread_local RigScratch g_rigA;
+thread_local unsigned long long g_rigHostPoints = 0;  // points the last call resolved on the host
+constexpr unsigned long long kUndecidedCapacity = 1ull << 16;  // list entries kept between calls (grown on demand)
+constexpr int kThreads = 256;
+
+// Lists point `index` for the host
+__device__ __forceinline__ void listPoint(unsigned long long index, unsigned long long* list, unsigned long long cap,
+                                          unsigned long long* count) {
+  const unsigned long long slot = atomicAdd(count, 1ull);
+  if (slot < cap) list[slot] = index;
+}
+
+// main's coverage loop: thread (j, k) counts the cameras that see distances[k] * samples[j] into hist[k][count]; one
+// atomic per distinct count in the warp
+__global__ void __launch_bounds__(kThreads) coverageKernel(const DevCamera* __restrict__ cams, int n,
+                                                           const double* __restrict__ samples, int numSamples,
+                                                           const double* __restrict__ distances,
+                                                           unsigned long long* __restrict__ hist,
+                                                           unsigned long long* list, unsigned long long cap,
+                                                           unsigned long long* count) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, k = blockIdx.y;
+  if (j >= numSamples) return;
+  const double d = distances[k];
+  const int c = provenCount<false>(cams, n, d * samples[3 * j], d * samples[3 * j + 1], d * samples[3 * j + 2], nullptr);
+  if (c < 0) listPoint((unsigned long long)k << 32 | (unsigned)j, list, cap, count);
+  const unsigned peers = __match_any_sync(__activemask(), c);
+  if (c >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1)
+    atomicAdd(&hist[(size_t)k * (n + 1) + c], (unsigned long long)__popc(peers));
+}
+
+// saveEquirect's pixel (x, y): (cos(lat) cos(lon), cos(lat) sin(lon), sin(lat)) * distance from the host's tables
+// tabs = {cosLat[H], sinLat[H], cosLon[W], sinLon[W]}; undecided pixels are written -1 / 0 and listed
+__global__ void __launch_bounds__(kThreads) equirectKernel(const DevCamera* __restrict__ cams, int n, int W, int H,
+                                                           const double* __restrict__ tabs, double distance,
+                                                           int32_t* __restrict__ counts, float* __restrict__ timing,
+                                                           unsigned long long* list, unsigned long long cap,
+                                                           unsigned long long* count) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= W) return;
+  const double cl = tabs[y], sl = tabs[H + y], co = tabs[2 * H + x], so = tabs[2 * H + W + x];
+  const double px = cl * co * distance, py = cl * so * distance, pz = sl * distance;
+  const size_t at = (size_t)y * W + x;
+  float m = 1.0f;
+  const int c = timing ? provenCount<true>(cams, n, px, py, pz, &m) : provenCount<false>(cams, n, px, py, pz, nullptr);
+  if (c < 0) listPoint(at, list, cap, count);
+  counts[at] = c;
+  if (timing) timing[at] = m;
+}
+
+// saveCamera's pixel (x, y) of camera `cam`: 0 outside its image circle (edge2 from the host), else the cameras that
+// see the interval of cam.rig({x + .5, y + .5}, distance)
+__global__ void __launch_bounds__(kThreads) cameraKernel(const DevCamera* __restrict__ cams, int n, int cam,
+                                                         double edge2, int W, int H, double distance,
+                                                         int32_t* __restrict__ counts, unsigned long long* list,
+                                                         unsigned long long cap, unsigned long long* count) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= W) return;
+  const size_t at = (size_t)y * W + x;
+  const DevCamera& c = cams[cam];
+  if (!c.defaultFov) {
+    const double sx = (x + 0.5 - c.principal[0]) / c.focal[0], sy = (y + 0.5 - c.principal[1]) / c.focal[1];
+    if (sx * sx + sy * sy >= edge2) {
+      counts[at] = 0;
+      return;
+    }
+  }
+  Iv w[3];
+  rigPointIv(c, x, y, distance, w);
+  int total = 0;
+  for (int i = 0; i < n; ++i) {
+    Iv py;
+    const int s = seesIv(cams[i], w, &py);
+    if (s == kUndecided) {
+      total = -1;
+      listPoint(at, list, cap, count);
+      break;
+    }
+    total += s;
+  }
+  counts[at] = total;
+}
+
+// saveCrossSection's point (x + .5 - .5 dim, y + .5 - .5 dim, 0), exact
+__global__ void __launch_bounds__(kThreads) crossSectionKernel(const DevCamera* __restrict__ cams, int n, int dim,
+                                                               int32_t* __restrict__ counts, unsigned long long* list,
+                                                               unsigned long long cap, unsigned long long* count) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= dim) return;
+  const size_t at = (size_t)y * dim + x;
+  const int c = provenCount<false>(cams, n, x + 0.5 - 0.5 * dim, y + 0.5 - 0.5 * dim, 0.0, nullptr);
+  if (c < 0) listPoint(at, list, cap, count);
+  counts[at] = c;
+}
+
+// Writes the host's values of the listed pixels
+__global__ void resolveKernel(const unsigned long long* __restrict__ list, const int32_t* __restrict__ c,
+                              const float* __restrict__ t, int num, int32_t* counts, float* timing) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= num) return;
+  counts[list[k]] = c[k];
+  if (timing) timing[list[k]] = t[k];
+}
+
+// Cameras as the caller holds them, with rotation9's rotation when given
+int rigCameras(const char* who, const DerpCameraDesc* cams, const double* rotation9, int n, std::vector<DevCamera>& out) {
+  if (!cams || n < 1) return fail(DERP_EINVAL, std::string(who) + ": at least one camera is required");
+  out.resize(n);
+  for (int i = 0; i < n; ++i) {
+    if (!host::makeCamera(cams[i], &out[i])) return fail(DERP_EINVAL, std::string(who) + ": invalid camera " + std::to_string(i));
+    if (rotation9)
+      for (int k = 0; k < 9; ++k) out[i].rot[k] = rotation9[9 * i + k];
+  }
+  return DERP_OK;
+}
+
+int checkGrid(const char* who, long long w, long long h) {
+  if (w < 1 || h < 1 || h > 65535 || w * h >= (1ll << 31))
+    return fail(DERP_EINVAL, std::string(who) + ": the grid must have 1..65535 rows and fewer than 2^31 points");
+  return DERP_OK;
+}
+
+// The equirect's sample tables {cosLat[H], sinLat[H], cosLon[W], sinLon[W]} (RigAnalyzer.cpp:393-397)
+std::vector<double> equirectTables(int W, int H) {
+  std::vector<double> t(2 * (size_t)H + 2 * (size_t)W);
+  for (int y = 0; y < H; ++y) {
+    const double lat = M_PI / 2 - (y + 0.5) / H * M_PI;
+    t[y] = cos(lat);
+    t[H + y] = sin(lat);
+  }
+  for (int x = 0; x < W; ++x) {
+    const double lon = -M_PI + (x + 0.5) / W * 2 * M_PI;
+    t[2 * H + x] = cos(lon);
+    t[2 * H + W + x] = sin(lon);
+  }
+  return t;
+}
+
+// Launches `run(list, cap, count)` until the undecided list holds every listed point (the decisions are deterministic,
+// so a second launch lists the same points) and returns the list in host memory
+template <class Run>
+int runListed(Run run, std::vector<unsigned long long>& list) {
+  RigScratch& g = g_rigA;
+  CU(g.count.ensure(1));
+  CU(g.undecided.ensure(kUndecidedCapacity));
+  unsigned long long count = 0;
+  for (;;) {
+    CU(cudaMemset(g.count.p, 0, sizeof count));
+    if (int rc = run(g.undecided.p, (unsigned long long)g.undecided.n, g.count.p)) return rc;
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(&count, g.count.p, sizeof count, cudaMemcpyDeviceToHost));
+    if (count <= g.undecided.n) break;
+    CU(g.undecided.ensure(count));
+  }
+  list.resize(count);
+  if (count) CU(cudaMemcpy(list.data(), g.undecided.p, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  g_rigHostPoints = count;
+  return DERP_OK;
+}
+
+// Writes the host's values c (and t) of the listed pixels into the device planes
+int resolvePixels(const std::vector<unsigned long long>& list, const std::vector<int32_t>& c,
+                  const std::vector<float>* t, int32_t* counts, float* timing) {
+  if (list.empty()) return DERP_OK;
+  RigScratch& g = g_rigA;
+  if (int rc = upload(g.resolvedCounts, c.data(), c.size())) return rc;
+  if (t)
+    if (int rc = upload(g.resolvedTiming, t->data(), t->size())) return rc;
+  resolveKernel<<<grid1(list.size()), 256>>>(g.undecided.p, g.resolvedCounts.p, t ? g.resolvedTiming.p : nullptr,
+                                             (int)list.size(), counts, timing);
+  CU(cudaGetLastError());
+  return DERP_OK;
+}
+
+int uploadCams(const std::vector<DevCamera>& c) { return upload(g_rigA.cams, c.data(), c.size()); }
+
+}  // namespace
+
+extern "C" {
+
+int derp_rig_coverage(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams,
+                      const double* samples, int num_samples, const double* distances, int num_distances,
+                      uint64_t* hist) {
+  static const char* who = "derp_rig_coverage";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (!samples || !distances || !hist || num_samples < 1 || num_distances < 1 || num_distances > 65535)
+    return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
+  CU(cudaSetDevice(device));
+  RigScratch& g = g_rigA;
+  if (int rc = uploadCams(c)) return rc;
+  if (int rc = upload(g.tabs, samples, 3 * (size_t)num_samples)) return rc;
+  DevBuf<double> dist;
+  if (int rc = upload(dist, distances, num_distances)) return rc;
+  const size_t nh = (size_t)num_distances * (num_cams + 1);
+  CU(g.hist.ensure(nh));
+  CU(cudaMemset(g.hist.p, 0, nh * sizeof(unsigned long long)));
+  std::vector<unsigned long long> list;
+  const dim3 grid(grid1(num_samples, kThreads), num_distances);
+  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
+    CU(cudaMemset(g.hist.p, 0, nh * sizeof(unsigned long long)));
+    coverageKernel<<<grid, kThreads>>>(g.cams.p, num_cams, g.tabs.p, num_samples, dist.p, g.hist.p, l, cap, count);
+    return DERP_OK;
+  };
+  if (int rc = runListed(run, list)) return rc;
+  std::vector<unsigned long long> h(nh);
+  CU(cudaMemcpy(h.data(), g.hist.p, nh * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  for (unsigned long long e : list) {
+    const int k = (int)(e >> 32), j = (int)(unsigned)e;
+    const double d = distances[k];
+    ++h[(size_t)k * (num_cams + 1) + countSees(c.data(), num_cams, d * samples[3 * j], d * samples[3 * j + 1],
+                                               d * samples[3 * j + 2])];
+  }
+  CU(cudaMemcpy(hist, h.data(), nh * sizeof(uint64_t), cudaMemcpyDefault));
+  return DERP_OK;
+}
+
+int derp_rig_equirect_coverage(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams, int width,
+                               int height, double distance, int32_t* counts, float* min_timing) {
+  static const char* who = "derp_rig_equirect_coverage";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (int rc = checkGrid(who, width, height)) return rc;
+  if (!counts) return fail(DERP_EINVAL, std::string(who) + ": counts is required");
+  CU(cudaSetDevice(device));
+  RigScratch& g = g_rigA;
+  if (int rc = uploadCams(c)) return rc;
+  const std::vector<double> tabs = equirectTables(width, height);
+  if (int rc = upload(g.tabs, tabs.data(), tabs.size())) return rc;
+  const size_t np = (size_t)width * height;
+  int32_t* dc = counts;
+  float* dt = min_timing;
+  if (int rc = outBuffer(dc, np, g.counts)) return rc;
+  if (dt)
+    if (int rc = outBuffer(dt, np, g.timing)) return rc;
+  std::vector<unsigned long long> list;
+  const dim3 grid(grid1(width, kThreads), height);
+  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
+    equirectKernel<<<grid, kThreads>>>(g.cams.p, num_cams, width, height, g.tabs.p, distance, dc, dt, l, cap, count);
+    return DERP_OK;
+  };
+  if (int rc = runListed(run, list)) return rc;
+  std::vector<int32_t> rc(list.size());
+  std::vector<float> rt(list.size()), scratch(num_cams);
+  for (size_t k = 0; k < list.size(); ++k) {
+    const int x = (int)(list[k] % width), y = (int)(list[k] / width);
+    const double cl = tabs[y], sl = tabs[height + y], co = tabs[2 * height + x], so = tabs[2 * height + width + x];
+    double m;
+    rc[k] = countTiming(c.data(), num_cams, cl * co * distance, cl * so * distance, sl * distance, scratch.data(), &m);
+    rt[k] = (float)m;
+  }
+  if (int e = resolvePixels(list, rc, dt ? &rt : nullptr, dc, dt)) return e;
+  if (int e = stageOut(counts, dc, np)) return e;
+  if (dt)
+    if (int e = stageOut(min_timing, dt, np)) return e;
+  return DERP_OK;
+}
+
+int derp_rig_camera_coverage(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams, int cam,
+                             double distance, int32_t* counts) {
+  static const char* who = "derp_rig_camera_coverage";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (cam < 0 || cam >= num_cams || !counts) return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
+  const int W = (int)c[cam].res[0], H = (int)c[cam].res[1];  // kDimX = int(resolution.x())
+  if (int rc = checkGrid(who, W, H)) return rc;
+  const double edge2 = c[cam].defaultFov ? 0 : imageCircleEdge2(c[cam]);
+  CU(cudaSetDevice(device));
+  RigScratch& g = g_rigA;
+  if (int rc = uploadCams(c)) return rc;
+  const size_t np = (size_t)W * H;
+  int32_t* dc = counts;
+  if (int rc = outBuffer(dc, np, g.counts)) return rc;
+  std::vector<unsigned long long> list;
+  const dim3 grid(grid1(W, kThreads), H);
+  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
+    cameraKernel<<<grid, kThreads>>>(g.cams.p, num_cams, cam, edge2, W, H, distance, dc, l, cap, count);
+    return DERP_OK;
+  };
+  if (int rc = runListed(run, list)) return rc;
+  std::vector<int32_t> rc(list.size());
+  for (size_t k = 0; k < list.size(); ++k)
+    rc[k] = countCameraPixel(c.data(), num_cams, cam, edge2, (int)(list[k] % W), (int)(list[k] / W), distance);
+  if (int e = resolvePixels(list, rc, nullptr, dc, nullptr)) return e;
+  return stageOut(counts, dc, np);
+}
+
+int derp_rig_cross_section(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams, int dim,
+                           int32_t* counts) {
+  static const char* who = "derp_rig_cross_section";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (int rc = checkGrid(who, dim, dim)) return rc;
+  if (!counts) return fail(DERP_EINVAL, std::string(who) + ": counts is required");
+  CU(cudaSetDevice(device));
+  RigScratch& g = g_rigA;
+  if (int rc = uploadCams(c)) return rc;
+  const size_t np = (size_t)dim * dim;
+  int32_t* dc = counts;
+  if (int rc = outBuffer(dc, np, g.counts)) return rc;
+  std::vector<unsigned long long> list;
+  const dim3 grid(grid1(dim, kThreads), dim);
+  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
+    crossSectionKernel<<<grid, kThreads>>>(g.cams.p, num_cams, dim, dc, l, cap, count);
+    return DERP_OK;
+  };
+  if (int rc = runListed(run, list)) return rc;
+  std::vector<int32_t> rc(list.size());
+  for (size_t k = 0; k < list.size(); ++k)
+    rc[k] = countSees(c.data(), num_cams, (int)(list[k] % dim) + 0.5 - 0.5 * dim, (int)(list[k] / dim) + 0.5 - 0.5 * dim,
+                      0.0);
+  if (int e = resolvePixels(list, rc, nullptr, dc, nullptr)) return e;
+  return stageOut(counts, dc, np);
+}
+
+uint64_t derp_rig_analysis_last_host_points(void) { return g_rigHostPoints; }
+
+int derp_test_rig_coverage_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams,
+                                const double* samples, int num_samples, const double* distances, int num_distances,
+                                uint64_t* hist) {
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras("derp_test_rig_coverage_host", cams, rotation9, num_cams, c)) return rc;
+  if (!samples || !distances || !hist || num_samples < 1 || num_distances < 1) return fail(DERP_EINVAL, "bad arguments");
+  std::fill(hist, hist + (size_t)num_distances * (num_cams + 1), 0);
+  for (int k = 0; k < num_distances; ++k)
+    for (int j = 0; j < num_samples; ++j) {
+      const double d = distances[k];
+      ++hist[(size_t)k * (num_cams + 1) +
+             countSees(c.data(), num_cams, d * samples[3 * j], d * samples[3 * j + 1], d * samples[3 * j + 2])];
+    }
+  return DERP_OK;
+}
+
+int derp_test_rig_equirect_coverage_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, int width,
+                                         int height, double distance, int32_t* counts, float* min_timing) {
+  static const char* who = "derp_test_rig_equirect_coverage_host";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (int rc = checkGrid(who, width, height)) return rc;
+  if (!counts) return fail(DERP_EINVAL, std::string(who) + ": counts is required");
+  const std::vector<double> t = equirectTables(width, height);
+  std::vector<float> scratch(num_cams);
+  for (int y = 0; y < height; ++y)
+    for (int x = 0; x < width; ++x) {
+      const double cl = t[y], sl = t[height + y], co = t[2 * height + x], so = t[2 * height + width + x];
+      double m;
+      const size_t at = (size_t)y * width + x;
+      counts[at] = countTiming(c.data(), num_cams, cl * co * distance, cl * so * distance, sl * distance,
+                               scratch.data(), &m);
+      if (min_timing) min_timing[at] = (float)m;
+    }
+  return DERP_OK;
+}
+
+int derp_test_rig_camera_coverage_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, int cam,
+                                       double distance, int32_t* counts) {
+  static const char* who = "derp_test_rig_camera_coverage_host";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (cam < 0 || cam >= num_cams || !counts) return fail(DERP_EINVAL, std::string(who) + ": bad arguments");
+  const int W = (int)c[cam].res[0], H = (int)c[cam].res[1];
+  if (int rc = checkGrid(who, W, H)) return rc;
+  const double edge2 = c[cam].defaultFov ? 0 : imageCircleEdge2(c[cam]);
+  for (int y = 0; y < H; ++y)
+    for (int x = 0; x < W; ++x) counts[(size_t)y * W + x] = countCameraPixel(c.data(), num_cams, cam, edge2, x, y, distance);
+  return DERP_OK;
+}
+
+int derp_test_rig_cross_section_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, int dim,
+                                     int32_t* counts) {
+  static const char* who = "derp_test_rig_cross_section_host";
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras(who, cams, rotation9, num_cams, c)) return rc;
+  if (int rc = checkGrid(who, dim, dim)) return rc;
+  if (!counts) return fail(DERP_EINVAL, std::string(who) + ": counts is required");
+  for (int y = 0; y < dim; ++y)
+    for (int x = 0; x < dim; ++x)
+      counts[(size_t)y * dim + x] = countSees(c.data(), num_cams, x + 0.5 - 0.5 * dim, y + 0.5 - 0.5 * dim, 0.0);
+  return DERP_OK;
+}
+
+}  // extern "C"

@@ -185,7 +185,7 @@ int checkProject(const char* who, const DerpCameraDesc* cams, int n, double dept
 // The host's decision at pixel (x, y) of camera c: the mask index, or -1 (the same DERP_HD code with the C library)
 long long projectPixelHost(const DevCamera& c, int x, int y, double depth, int mw, int mh) {
   double w[3];
-  derp::sweep::rigPoint(c, x, y, depth, w);
+  derp::rigPoint(c, x, y, depth, w);
   return derp::sweep::eqrIndex(w[0], w[1], w[2], mw, mh);
 }
 

@@ -10,6 +10,7 @@
 #include "../../../include/derp_rigsim.h"
 #include "../derp_camera.cuh"
 #include "io.h"
+#include "rig_json.h"
 
 const std::string kUsage = R"(
   - Render an artificial scene as seen by the specified rig.
@@ -239,50 +240,17 @@ std::vector<SimCamera> icosahedron(int w, int h, int circleRadius, float circleF
 }
 
 // ---- --rig_out: Camera::saveRig with sorted keys and doubleNumDigits = 10 (folly's FIXED mode) ------------------------
-std::string fixed10(double v) {
-  char b[64];
-  snprintf(b, sizeof b, "%.10f", v);
-  return b;
-}
-std::string vec(const double* v, int n) {
-  std::string s = "[";
-  for (int i = 0; i < n; ++i) s += std::string(i ? ", " : "") + fixed10(v[i]);
-  return s + "]";
-}
 void saveRig(const std::string& path, const std::vector<SimCamera>& cams) {
-  static const char* kTypes[] = {"FTHETA", "RECTILINEAR", "EQUISOLID", "ORTHOGRAPHIC"};
-  std::string out = "{\n  \"cameras\": [";
+  std::vector<rigjson::Camera> out(cams.size());
   for (size_t i = 0; i < cams.size(); ++i) {
-    const SimCamera& c = cams[i];
     derp::DevCamera dc;
-    CHECK(derp::host::makeCamera(c.d, &dc)) << "invalid camera " << c.id;
-    double fwd[3], up[3], right[3];
-    for (int k = 0; k < 3; ++k) {
-      right[k] = dc.rot[k];
-      up[k] = dc.rot[3 + k];
-      fwd[k] = -dc.rot[6 + k];
-    }
-    std::vector<std::pair<std::string, std::string>> kv = {
-        {"focal", vec(c.d.focal, 2)},       {"forward", vec(fwd, 3)},  {"id", "\"" + c.id + "\""},
-        {"origin", vec(c.d.origin, 3)},     {"resolution", vec(c.d.resolution, 2)},
-        {"right", vec(right, 3)},           {"type", std::string("\"") + kTypes[c.d.type] + "\""},
-        {"up", vec(up, 3)},                 {"version", "1"}};
-    if (c.d.has_principal && (c.d.principal[0] != c.d.resolution[0] / 2 || c.d.principal[1] != c.d.resolution[1] / 2))
-      kv.push_back({"principal", vec(c.d.principal, 2)});
-    if (c.d.distortion[0] != 0 || c.d.distortion[1] != 0 || c.d.distortion[2] != 0)
-      kv.push_back({"distortion", vec(c.d.distortion, 3)});
-    if (!c.group.empty()) kv.push_back({"group", "\"" + c.group + "\""});
-    if (c.d.has_fov && !dc.defaultFov) kv.push_back({"fov", fixed10(c.d.fov)});
-    std::sort(kv.begin(), kv.end());
-    out += std::string(i ? "," : "") + "\n    {";
-    for (size_t k = 0; k < kv.size(); ++k)
-      out += std::string(k ? "," : "") + "\n      \"" + kv[k].first + "\": " + kv[k].second;
-    out += "\n    }";
+    CHECK(derp::host::makeCamera(cams[i].d, &dc)) << "invalid camera " << cams[i].id;
+    out[i].d = cams[i].d;
+    std::copy(dc.rot, dc.rot + 9, out[i].rot);
+    out[i].id = cams[i].id;
+    out[i].group = cams[i].group;
   }
-  out += "\n  ]\n}\n";
-  std::ofstream f(path);
-  CHECK(f.good()) << "cannot write " << path;
-  f << out;
+  rigjson::saveRig(path, out, {}, false);
 }
 
 // ---- images -----------------------------------------------------------------------------------------------------------

@@ -179,6 +179,7 @@ class JsonParser {
 struct Rig {
   std::vector<DerpCameraDesc> cams;
   std::vector<std::string> ids;
+  std::vector<std::string> groups;  // "" where the camera has none
 };
 
 inline double jnum(const Json& j) {
@@ -230,6 +231,8 @@ inline Rig loadRig(const std::string& path) {  // Camera::loadRig (Camera.cpp:24
     }
     rig.cams.push_back(d);
     rig.ids.push_back(c.at("id").str);
+    const Json* g = c.find("group");
+    rig.groups.push_back(g ? g->str : "");
   }
   return rig;
 }
