@@ -731,6 +731,8 @@ _SWEEP_SIGS = {
     "derp_project_equirect_masks": (C.c_int, [C.c_int, _p(CameraDesc), C.c_int, C.c_double, _p(C.c_void_p), C.c_void_p,
                                               _p(C.c_void_p)]),
     "derp_project_last_host_pixels": (C.c_uint64, []),
+    "derp_test_eqr_index_proven": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "derp_test_eqr_index_host": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
 }
 # derp_test_sweep_*_host: the same arguments as the entry point without the device
 _SWEEP_HOST_SIGS = {"derp_test_sweep_%s_host" % k: (C.c_int, _SWEEP_SIGS["derp_sweep_" + k][1][1:])
@@ -846,6 +848,18 @@ class SweepView(_Binding):
             self._check(self.lib.derp_project_equirect_masks(device, *args))
         return outs
 
+    def eqr_index(self, pts_or_boxes, width, height, proven=False, device=0):
+        """int64 [n]: eqrIndex of points [n, 3] on the host (the index or -1), or with ``proven`` the device's
+        eqrIndexProven of boxes [n, 6] (x lo, x hi, y lo, y hi, z lo, z hi; -2 where it does not decide)."""
+        a = np.ascontiguousarray(pts_or_boxes, np.float64).reshape(-1, 6 if proven else 3)
+        out = np.empty(len(a), np.int64)
+        if proven:
+            self._check(self.lib.derp_test_eqr_index_proven(device, a.ctypes.data, len(a), width, height,
+                                                            out.ctypes.data))
+        else:
+            self._check(self.lib.derp_test_eqr_index_host(a.ctypes.data, len(a), width, height, out.ctypes.data))
+        return out
+
     def last_host_pixels(self):
         """Pixels this thread's last project_masks call resolved on the host (the device could not prove them)."""
         return int(self.lib.derp_project_last_host_pixels())
@@ -945,6 +959,8 @@ _RIGSIM_SIGS = {
     "derp_rigsim_last_rays": (C.c_uint64, []),
     "derp_rigsim_trace_host": (C.c_int, [C.c_void_p, _p(RigsimRender), C.c_void_p, C.c_int, C.c_void_p]),
     "derp_test_rigsim_area": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "derp_test_sky_texel": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "derp_test_sky_texel_host": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
 }
 RIGSIM_SYMBOLS = sorted(k for k in _RIGSIM_SIGS if k.startswith("derp_rigsim_"))
 
@@ -1042,6 +1058,17 @@ class RigSim(_Binding):
         """(rays whose sky texel the host resolved, supersample rays traced) in this thread's last render."""
         return int(self.lib.derp_rigsim_last_host_rays()), int(self.lib.derp_rigsim_last_rays())
 
+    def sky_texel(self, dirs, rows, cols, host=False, device=0):
+        """int32 [n, 2] (row, column) of float32 directions [n, 3] in a rows x cols skybox: the device's proven texel
+        ((-1, -1) where it leaves the ray to the host), or with ``host`` the C library's."""
+        d = np.ascontiguousarray(dirs, np.float32).reshape(-1, 3)
+        out = np.empty((len(d), 2), np.int32)
+        if host:
+            self._check(self.lib.derp_test_sky_texel_host(d.ctypes.data, len(d), rows, cols, out.ctypes.data))
+        else:
+            self._check(self.lib.derp_test_sky_texel(device, d.ctypes.data, len(d), rows, cols, out.ctypes.data))
+        return out
+
     def trace_host(self, scene, rays, skybox, **opts):
         """traceRayToGetColor on the host for float32 rays [n, 6] (origin, direction): float32 [n, 4] = B, G, R, depth."""
         o, keep = self.render_opts(skybox, **opts)
@@ -1069,7 +1096,17 @@ _RIGANALYSIS_SIGS = {
     "derp_test_rig_camera_coverage_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_double,
                                                      C.c_void_p]),
     "derp_test_rig_cross_section_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "derp_test_math": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "derp_test_acosf_exhaustive": (C.c_int, [C.c_int, C.c_void_p]),
+    "derp_test_rig_point_iv": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_double, C.c_void_p]),
+    "derp_test_sees_iv": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "derp_test_sees_device": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "derp_test_proven_count": (C.c_int, [C.c_int, _p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_void_p]),
+    "derp_test_count_timing_host": (C.c_int, [_p(CameraDesc), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                              C.c_void_p]),
 }
+MATH_FNS = {"sin": 0, "cos": 1, "atan": 2, "asin": 3, "atan2": 4, "acosf": 5, "atan2f": 6, "atan2Pos": 7}
 RIGANALYSIS_SYMBOLS = sorted(k for k in _RIGANALYSIS_SIGS if k.startswith("derp_rig_"))
 
 
@@ -1148,3 +1185,59 @@ class RigAnalysis(_Binding):
     def last_host_points(self):
         """The points this thread's last GPU call resolved on the host."""
         return int(self.lib.derp_rig_analysis_last_host_points())
+
+    # ---- probes of the device's interval proofs (derp_test_*) ----
+    def math(self, fn, a, b=None, device=0):
+        """The device's ``fn`` (a MATH_FNS name) of a (and b): float64 [n, 3] = value, widened interval lo, hi."""
+        a = np.ascontiguousarray(a, np.float64).ravel()
+        b = None if b is None else np.ascontiguousarray(b, np.float64).ravel()
+        out = np.empty((len(a), 3))
+        self._check(self.lib.derp_test_math(device, MATH_FNS[fn], a.ctypes.data, None if b is None else b.ctypes.data,
+                                            len(a), out.ctypes.data))
+        return out
+
+    def acosf_exhaustive(self, device=0):
+        """Every float in [-1, 1]: dict of the device's and host's greatest errors (ulps), their greatest distance in
+        float steps, and the host values outside the device value's widenF."""
+        st = np.zeros(4, np.uint32)
+        self._check(self.lib.derp_test_acosf_exhaustive(device, st.ctypes.data))
+        return {"device_ulps": st[0] / 2.0 ** 20, "host_ulps": st[1] / 2.0 ** 20, "steps": int(st[2]),
+                "outside": int(st[3])}
+
+    def rig_point_iv(self, desc, pix, depth, device=0):
+        """rigPointIv of int pixels [n, 2]: float64 [n, 7] = x lo, x hi, y lo, y hi, z lo, z hi, undistort's r."""
+        p = np.ascontiguousarray(pix, np.int32).reshape(-1, 2)
+        out = np.empty((len(p), 7))
+        self._check(self.lib.derp_test_rig_point_iv(device, C.byref(desc), p.ctypes.data, len(p), depth,
+                                                    out.ctypes.data))
+        return out
+
+    def sees_iv(self, desc, boxes, device=0):
+        """seesIv of boxes [n, 6] (x lo, x hi, y lo, y hi, z lo, z hi): (int32 decision 1 / 0 / -1, float64 py [n, 2])."""
+        b = np.ascontiguousarray(boxes, np.float64).reshape(-1, 6)
+        dec, py = np.empty(len(b), np.int32), np.empty((len(b), 2))
+        self._check(self.lib.derp_test_sees_iv(device, C.byref(desc), b.ctypes.data, len(b), dec.ctypes.data,
+                                               py.ctypes.data))
+        return dec, py
+
+    def sees_device(self, desc, pts, device=0):
+        """The device's Camera::sees of points [n, 3]: (float64 pixel [n, 2], bool seen [n])."""
+        p = np.ascontiguousarray(pts, np.float64).reshape(-1, 3)
+        pix, seen = np.empty((len(p), 2)), np.empty(len(p), np.uint8)
+        self._check(self.lib.derp_test_sees_device(device, C.byref(desc), p.ctypes.data, len(p), pix.ctypes.data,
+                                                   seen.ctypes.data))
+        return pix, seen.astype(bool)
+
+    def proven_count(self, descs, pts, rot=None, host=False, device=0):
+        """provenCount<true> of points [n, 3] (count -1: left to the host), or with ``host`` its host twin
+        countTiming: (int32 counts [n], float32 minTimingDiff [n])."""
+        descs, keep, r = self._rig(descs, rot)
+        p = np.ascontiguousarray(pts, np.float64).reshape(-1, 3)
+        counts, timing = np.empty(len(p), np.int32), np.empty(len(p), np.float32)
+        if host:
+            self._check(self.lib.derp_test_count_timing_host(descs, r, len(descs), p.ctypes.data, len(p),
+                                                             counts.ctypes.data, timing.ctypes.data))
+        else:
+            self._check(self.lib.derp_test_proven_count(device, descs, r, len(descs), p.ctypes.data, len(p),
+                                                        counts.ctypes.data, timing.ctypes.data))
+        return counts, timing

@@ -324,8 +324,9 @@ DERP_HD double undistort(const DevCamera& c, double y) {  // Camera.h:243-284
 // Device version: one division + fdlibm's degree-11 minimax polynomial (|t| <= tan(pi/8) after folding the
 // argument with atan(a/b) = pi/4 + atan((a-b)/(a+b))), coefficients as constant-bank operands.  CUDA's
 // libdevice atan2 materialises ~25 64-bit immediates with two UMOVs each inside the sweep's inner loop
-// (visible in the SASS); this one issues ~45 instructions in total.  Error < 1.5 ulp, i.e. the same
-// tolerance class as CUDA-vs-glibc atan2 (the value is narrowed to fp32 pixel coordinates afterwards).
+// (visible in the SASS); this one issues ~45 instructions in total.  Error < 2 ulp of the exact value (1.69
+// the largest measured, tests/test_gpu_interval_proofs.py), the bound of CUDA's own atan2 (the value is narrowed to
+// fp32 pixel coordinates afterwards; no proof widens it).
 #if defined(__CUDACC__)
 static __constant__ double kAtanT[11] = {  // static: one copy per translation unit that includes this header
     3.33333333333329318027e-01,  -1.99999999998764832476e-01, 1.42857142725034663711e-01,

@@ -1,6 +1,9 @@
 // include/derp_riganalysis.h: RigAnalyzer's coverage counts on sm_90a (per-point code and proof in
 // derp_riganalysis.cuh), the host resolution of the points the device leaves undecided, and the host instantiation of
 // the per-point code for the CPU tests.
+#include <cstring>
+#include <thread>
+
 #include "derp_host.cuh"
 #include "derp_riganalysis.cuh"
 #include "../../include/derp_riganalysis.h"
@@ -191,6 +194,126 @@ int resolvePixels(const std::vector<unsigned long long>& list, const std::vector
 }
 
 int uploadCams(const std::vector<DevCamera>& c) { return upload(g_rigA.cams, c.data(), c.size()); }
+
+// ---- test probes: the proofs' device functions on caller-given inputs ------------------------------------------------
+// The device's math function `fn` (derp_test_math) and its interval as the proofs widen it
+__global__ void mathProbeKernel(int fn, const double* a, const double* b, int n, double* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double v;
+  Iv w;
+  switch (fn) {
+    case DERP_MATH_SIN: w = widenD(v = sin(a[i]), kSinUlps, 0); break;
+    case DERP_MATH_COS: w = widenD(v = cos(a[i]), kSinUlps, 0); break;
+    case DERP_MATH_ATAN: w = widenD(v = atan(a[i]), kAtanUlps, 0); break;
+    case DERP_MATH_ASIN: w = widenD(v = asin(a[i]), kAtanUlps, 0); break;
+    case DERP_MATH_ATAN2: w = widenD(v = atan2(a[i], b[i]), kAtan2Ulps, 0); break;
+    case DERP_MATH_ACOSF: {
+      const float f = acosf((float)a[i]);
+      w = widenF(f, kAcosfUlps);
+      v = f;
+      break;
+    }
+    case DERP_MATH_ATAN2F: {
+      const float f = atan2f((float)a[i], (float)b[i]);
+      w = widenF(f, kAtan2fUlps);
+      v = f;
+      break;
+    }
+    default: w = Iv{v = atan2Pos(a[i], b[i]), v}; break;
+  }
+  out[3 * i] = v;
+  out[3 * i + 1] = w.lo;
+  out[3 * i + 2] = w.hi;
+}
+
+// Every float x in [first, first + count) (bit patterns) against the host's acosf(x) and acos(double(x)) (ref): the
+// greatest device and host errors in ulps of ref (x 2^20), the greatest distance in float steps between the two, and
+// the number of host values outside widenF of the device's
+__global__ void acosfCheckKernel(uint32_t first, uint32_t count, const float* __restrict__ host,
+                                 const double* __restrict__ ref, unsigned* stats) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned devErr = 0, hostErr = 0, steps = 0, outside = 0;
+  if (i < count) {
+    const float x = __uint_as_float(first + i), d = acosf(x), h = host[i];
+    const double r = ref[i];
+    int e;
+    frexp(r, &e);
+    const double ulp = ldexp(1.0, max(e - 24, -149));
+    devErr = (unsigned)fmin(fabs(d - r) / ulp * 0x1p20, 4294967295.0);
+    hostErr = (unsigned)fmin(fabs(h - r) / ulp * 0x1p20, 4294967295.0);
+    const int bd = __float_as_int(d), bh = __float_as_int(h);  // acos >= 0: bit patterns order the values
+    steps = (unsigned)abs(bd - bh);
+    const Iv w = widenF(d, kAcosfUlps);
+    outside = !(w.lo <= h && h <= w.hi);
+  }
+  const unsigned m = __activemask();
+  devErr = __reduce_max_sync(m, devErr);
+  hostErr = __reduce_max_sync(m, hostErr);
+  steps = __reduce_max_sync(m, steps);
+  outside = __reduce_add_sync(m, outside);
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(&stats[0], devErr);
+    atomicMax(&stats[1], hostErr);
+    atomicMax(&stats[2], steps);
+    atomicAdd(&stats[3], outside);
+  }
+}
+
+__global__ void rigPointIvKernel(DevCamera c, const int32_t* pix, int n, double depth, double* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Iv w[3];
+  rigPointIv(c, pix[2 * i], pix[2 * i + 1], depth, w);
+  for (int k = 0; k < 3; ++k) {
+    out[7 * i + 2 * k] = w[k].lo;
+    out[7 * i + 2 * k + 1] = w[k].hi;
+  }
+  const double sx = (pix[2 * i] + 0.5 - c.principal[0]) / c.focal[0];
+  const double sy = (pix[2 * i + 1] + 0.5 - c.principal[1]) / c.focal[1];
+  out[7 * i + 6] = undistort(c, sqrt(sx * sx + sy * sy));
+}
+
+__global__ void seesIvKernel(DevCamera c, const double* box, int n, int32_t* decision, double* py) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Iv w[3] = {{box[6 * i], box[6 * i + 1]}, {box[6 * i + 2], box[6 * i + 3]}, {box[6 * i + 4], box[6 * i + 5]}};
+  Iv y{NAN, NAN};
+  decision[i] = seesIv(c, w, &y);
+  py[2 * i] = y.lo;
+  py[2 * i + 1] = y.hi;
+}
+
+__global__ void seesKernel(DevCamera c, const double* pts, int n, double* pix, uint8_t* seen) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double x = NAN, y = NAN;
+  seen[i] = sees(c, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], &x, &y);
+  pix[2 * i] = x;
+  pix[2 * i + 1] = y;
+}
+
+__global__ void provenCountKernel(const DevCamera* cams, int num, const double* pts, int n, int32_t* counts,
+                                  float* timing) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float m = NAN;
+  counts[i] = provenCount<true>(cams, num, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], &m);
+  timing[i] = m;
+}
+
+int probeCamera(const DerpCameraDesc* d, DevCamera* c) {
+  if (!d || !host::makeCamera(*d, c)) return fail(DERP_EINVAL, "invalid camera");
+  return DERP_OK;
+}
+
+// Copies n elements of a device buffer to the caller's host array
+template <typename T>
+int download(T* dst, const DevBuf<T>& src, size_t n) {
+  CU(cudaGetLastError());
+  CU(cudaMemcpy(dst, src.p, n * sizeof(T), cudaMemcpyDeviceToHost));
+  return DERP_OK;
+}
 
 }  // namespace
 
@@ -394,6 +517,133 @@ int derp_test_rig_cross_section_host(const DerpCameraDesc* cams, const double* r
   for (int y = 0; y < dim; ++y)
     for (int x = 0; x < dim; ++x)
       counts[(size_t)y * dim + x] = countSees(c.data(), num_cams, x + 0.5 - 0.5 * dim, y + 0.5 - 0.5 * dim, 0.0);
+  return DERP_OK;
+}
+
+int derp_test_math(int device, int fn, const double* a, const double* b, int n, double* out) {
+  const bool two = fn == DERP_MATH_ATAN2 || fn == DERP_MATH_ATAN2F || fn == DERP_MATH_ATAN2POS;
+  if (fn < DERP_MATH_SIN || fn > DERP_MATH_ATAN2POS || !a || (two && !b) || n < 1 || !out)
+    return fail(DERP_EINVAL, "derp_test_math: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<double> da, db, dout;
+  if (int rc = upload(da, a, n)) return rc;
+  if (two)
+    if (int rc = upload(db, b, n)) return rc;
+  CU(dout.ensure(3 * (size_t)n));
+  mathProbeKernel<<<grid1(n), 256>>>(fn, da.p, db.p, n, dout.p);
+  return download(out, dout, 3 * (size_t)n);
+}
+
+int derp_test_acosf_exhaustive(int device, uint32_t* stats) {
+  if (!stats) return fail(DERP_EINVAL, "derp_test_acosf_exhaustive: bad arguments");
+  CU(cudaSetDevice(device));
+  constexpr uint32_t kChunk = 1u << 25;
+  DevBuf<float> dh;
+  DevBuf<double> dr;
+  DevBuf<unsigned> ds;
+  CU(dh.ensure(kChunk));
+  CU(dr.ensure(kChunk));
+  CU(ds.ensure(4));
+  CU(cudaMemset(ds.p, 0, 4 * sizeof(unsigned)));
+  std::vector<float> h(kChunk);
+  std::vector<double> r(kChunk);
+  const unsigned nt = std::max(1u, std::thread::hardware_concurrency());
+  for (const uint32_t sign : {0u, 0x80000000u})  // [+0, 1] and [-0, -1]: bit patterns up to 1.0f's
+    for (uint32_t first = 0; first <= 0x3f800000u; first += kChunk) {
+      const uint32_t count = std::min<uint32_t>(kChunk, 0x3f800001u - first);
+      std::vector<std::thread> pool;
+      for (unsigned t = 0; t < nt; ++t)
+        pool.emplace_back([&, t] {
+          for (uint32_t i = t; i < count; i += nt) {
+            const uint32_t bits = (sign | first) + i;
+            float x;
+            memcpy(&x, &bits, 4);
+            h[i] = acosf(x);
+            r[i] = acos((double)x);
+          }
+        });
+      for (auto& p : pool) p.join();
+      CU(cudaMemcpy(dh.p, h.data(), count * sizeof(float), cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(dr.p, r.data(), count * sizeof(double), cudaMemcpyHostToDevice));
+      acosfCheckKernel<<<grid1(count), 256>>>(sign | first, count, dh.p, dr.p, ds.p);
+    }
+  return download(stats, ds, 4);
+}
+
+int derp_test_rig_point_iv(int device, const DerpCameraDesc* cam, const int32_t* pix, int n, double depth, double* out) {
+  DevCamera c;
+  if (int rc = probeCamera(cam, &c)) return rc;
+  if (!pix || n < 1 || !out) return fail(DERP_EINVAL, "derp_test_rig_point_iv: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<int32_t> dp;
+  DevBuf<double> dout;
+  if (int rc = upload(dp, pix, 2 * (size_t)n)) return rc;
+  CU(dout.ensure(7 * (size_t)n));
+  rigPointIvKernel<<<grid1(n), 256>>>(c, dp.p, n, depth, dout.p);
+  return download(out, dout, 7 * (size_t)n);
+}
+
+int derp_test_sees_iv(int device, const DerpCameraDesc* cam, const double* boxes, int n, int32_t* decision,
+                      double* py) {
+  DevCamera c;
+  if (int rc = probeCamera(cam, &c)) return rc;
+  if (!boxes || n < 1 || !decision || !py) return fail(DERP_EINVAL, "derp_test_sees_iv: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<double> db, dy;
+  DevBuf<int32_t> dd;
+  if (int rc = upload(db, boxes, 6 * (size_t)n)) return rc;
+  CU(dd.ensure(n));
+  CU(dy.ensure(2 * (size_t)n));
+  seesIvKernel<<<grid1(n), 256>>>(c, db.p, n, dd.p, dy.p);
+  if (int rc = download(decision, dd, n)) return rc;
+  return download(py, dy, 2 * (size_t)n);
+}
+
+int derp_test_sees_device(int device, const DerpCameraDesc* cam, const double* pts, int n, double* pix, uint8_t* seen) {
+  DevCamera c;
+  if (int rc = probeCamera(cam, &c)) return rc;
+  if (!pts || n < 1 || !pix || !seen) return fail(DERP_EINVAL, "derp_test_sees_device: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<double> dp, dx;
+  DevBuf<uint8_t> ds;
+  if (int rc = upload(dp, pts, 3 * (size_t)n)) return rc;
+  CU(dx.ensure(2 * (size_t)n));
+  CU(ds.ensure(n));
+  seesKernel<<<grid1(n), 256>>>(c, dp.p, n, dx.p, ds.p);
+  if (int rc = download(pix, dx, 2 * (size_t)n)) return rc;
+  return download(seen, ds, n);
+}
+
+int derp_test_proven_count(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams,
+                           const double* pts, int n, int32_t* counts, float* timing) {
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras("derp_test_proven_count", cams, rotation9, num_cams, c)) return rc;
+  if (!pts || n < 1 || !counts || !timing) return fail(DERP_EINVAL, "derp_test_proven_count: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<DevCamera> dc;
+  DevBuf<double> dp;
+  DevBuf<int32_t> dn;
+  DevBuf<float> dt;
+  if (int rc = upload(dc, c.data(), c.size())) return rc;
+  if (int rc = upload(dp, pts, 3 * (size_t)n)) return rc;
+  CU(dn.ensure(n));
+  CU(dt.ensure(n));
+  provenCountKernel<<<grid1(n), 256>>>(dc.p, num_cams, dp.p, n, dn.p, dt.p);
+  if (int rc = download(counts, dn, n)) return rc;
+  return download(timing, dt, n);
+}
+
+int derp_test_count_timing_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, const double* pts,
+                                int n, int32_t* counts, float* timing) {
+  std::vector<DevCamera> c;
+  if (int rc = rigCameras("derp_test_count_timing_host", cams, rotation9, num_cams, c)) return rc;
+  if (!pts || n < 1 || !counts || !timing) return fail(DERP_EINVAL, "derp_test_count_timing_host: bad arguments");
+  std::vector<float> scratch(num_cams);
+  for (int i = 0; i < n; ++i) {
+    double m;
+    counts[i] = countTiming(c.data(), num_cams, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], scratch.data(), &m);
+    timing[i] = (float)m;
+  }
   return DERP_OK;
 }
 

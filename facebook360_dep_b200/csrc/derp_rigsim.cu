@@ -228,6 +228,16 @@ int downscaleInto(const float* src, int dw, int dh, int cn, int k, float* dst, D
   return stageOut(dst, d, n);
 }
 
+// Test probe: skyTexelDevice of the directions dirs[3 i .. 3 i + 2] into texel[2 i .. 2 i + 1], (-1, -1) when undecided
+__global__ void skyTexelKernel(const float* dirs, int n, int rows, int cols, int32_t* texel) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int row = -1, col = -1;
+  if (!skyTexelDevice(v3(dirs + 3 * i), rows, cols, &row, &col)) row = col = -1;
+  texel[2 * i] = row;
+  texel[2 * i + 1] = col;
+}
+
 }  // namespace
 
 extern "C" {
@@ -409,6 +419,25 @@ int derp_rigsim_trace_host(const DerpRigsimScene* scene, const DerpRigsimRender*
       skyColor(v, row, col, out + 4 * i);
     }
   }
+  return DERP_OK;
+}
+
+int derp_test_sky_texel(int device, const float* dirs, int n, int rows, int cols, int32_t* texel) {
+  if (!dirs || n < 1 || rows < 1 || cols < 1 || !texel) return fail(DERP_EINVAL, "derp_test_sky_texel: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<float> dd;
+  DevBuf<int32_t> dt;
+  if (int rc = upload(dd, dirs, 3 * (size_t)n)) return rc;
+  CU(dt.ensure(2 * (size_t)n));
+  skyTexelKernel<<<grid1(n), 256>>>(dd.p, n, rows, cols, dt.p);
+  CU(cudaGetLastError());
+  CU(cudaMemcpy(texel, dt.p, 2 * (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return DERP_OK;
+}
+
+int derp_test_sky_texel_host(const float* dirs, int n, int rows, int cols, int32_t* texel) {
+  if (!dirs || n < 1 || rows < 1 || cols < 1 || !texel) return fail(DERP_EINVAL, "derp_test_sky_texel_host: bad arguments");
+  for (int i = 0; i < n; ++i) skyTexelHost(v3(dirs + 3 * i), rows, cols, &texel[2 * i], &texel[2 * i + 1]);
   return DERP_OK;
 }
 

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "derp_camera.cuh"
+#include "derp_interval.cuh"
 #include "../../include/derp_rigsim.h"
 
 namespace derp {
@@ -207,22 +208,17 @@ inline void skyTexelHost(V3 d, int rows, int cols, int* row, int* col) {
 
 #if defined(__CUDACC__)
 // The device's acosf and atan2f are within 2 and 3 ulp of the exact value (CUDA C++ Programming Guide, "Mathematical
-// Functions", single precision); glibc's are within 1 and 2 ulp on x86_64 (the libm-test-ulps tables of the manual,
-// "Errors in Math Functions").  So the C library's value lies within kAcosUlp / kAtan2Ulp float steps of the device's.
-constexpr int kAcosUlp = 2 + 1, kAtan2Ulp = 3 + 2;
-__device__ __forceinline__ float stepsFrom(float v, int k, float toward) {
-  for (int i = 0; i < k; ++i) v = nextafterf(v, toward);
-  return v;
-}
-// The texel when both ends of the widened interval give the same row and column before the modulo (then every value
-// between does, the chain being monotone); false otherwise
+// Functions", single precision) and glibc's within the 2 derp_interval.cuh budgets.  Those are ulps of the exact value,
+// so the C library's value lies in widenF of the device's with kAcosfUlps / kAtan2fUlps, a relative bound plus 1 ulp.
+// (Counting float steps from the device's value would not do: just above a power of two, 2 ulp below the exact value
+// are 4 steps.)  The texel is decided when both ends of the widened intervals give the same row and column before the
+// modulo (then every value between does, the chain being monotone); false otherwise
 __device__ __forceinline__ bool skyTexelDevice(V3 d, int rows, int cols, int* row, int* col) {
   const float z = d.z < -1.0f ? -1.0f : d.z > 1.0f ? 1.0f : d.z;
-  const float p = acosf(z), a = atan2f(d.y, d.x);
+  const Iv p = ivFloat(widenF(acosf(z), kAcosfUlps)), a = ivFloat(widenF(atan2f(d.y, d.x), kAtan2fUlps));
   int r0, c0, r1, c1;
-  if (!skyTexelOf(stepsFrom(p, kAcosUlp, -INFINITY), stepsFrom(a, kAtan2Ulp, -INFINITY), rows, cols, &r0, &c0) ||
-      !skyTexelOf(stepsFrom(p, kAcosUlp, INFINITY), stepsFrom(a, kAtan2Ulp, INFINITY), rows, cols, &r1, &c1) ||
-      r0 != r1 || c0 != c1)
+  if (!skyTexelOf((float)p.lo, (float)a.lo, rows, cols, &r0, &c0) ||
+      !skyTexelOf((float)p.hi, (float)a.hi, rows, cols, &r1, &c1) || r0 != r1 || c0 != c1)
     return false;
   *row = r0;
   *col = c0 % cols;

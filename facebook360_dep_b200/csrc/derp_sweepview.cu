@@ -189,6 +189,14 @@ long long projectPixelHost(const DevCamera& c, int x, int y, double depth, int m
   return derp::sweep::eqrIndex(w[0], w[1], w[2], mw, mh);
 }
 
+// Test probe: eqrIndexProven of the boxes box[6 i .. 6 i + 5] (x lo, x hi, y lo, y hi, z lo, z hi)
+__global__ void eqrIndexProvenKernel(const double* box, int n, int W, int H, long long* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Iv w[3] = {{box[6 * i], box[6 * i + 1]}, {box[6 * i + 2], box[6 * i + 3]}, {box[6 * i + 4], box[6 * i + 5]}};
+  out[i] = derp::sweep::eqrIndexProven(w, W, H);
+}
+
 }  // namespace
 
 extern "C" {
@@ -476,6 +484,26 @@ int derp_test_sweep_equirect_host(const DerpCameraDesc* cams, int num_cams, int 
             depth * p.cosP[(size_t)k * p.pStride + y], bg, &hits);
       }
   }
+  return DERP_OK;
+}
+
+int derp_test_eqr_index_proven(int device, const double* boxes, int n, int width, int height, int64_t* out) {
+  if (!boxes || n < 1 || width < 1 || height < 1 || !out)
+    return fail(DERP_EINVAL, "derp_test_eqr_index_proven: bad arguments");
+  CU(cudaSetDevice(device));
+  DevBuf<double> db;
+  DevBuf<long long> dout;
+  if (int rc = upload(db, boxes, 6 * (size_t)n)) return rc;
+  CU(dout.ensure(n));
+  eqrIndexProvenKernel<<<grid1(n), 256>>>(db.p, n, width, height, dout.p);
+  CU(cudaGetLastError());
+  CU(cudaMemcpy(out, dout.p, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  return DERP_OK;
+}
+
+int derp_test_eqr_index_host(const double* pts, int n, int width, int height, int64_t* out) {
+  if (!pts || n < 1 || width < 1 || height < 1 || !out) return fail(DERP_EINVAL, "derp_test_eqr_index_host: bad arguments");
+  for (int i = 0; i < n; ++i) out[i] = derp::sweep::eqrIndex(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], width, height);
   return DERP_OK;
 }
 

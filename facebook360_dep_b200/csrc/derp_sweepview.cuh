@@ -250,6 +250,9 @@ __device__ __forceinline__ long long eqrIndexProven(const Iv* w, int W, int H) {
   const Iv phi = Iv{widenF(acosf((float)z.hi), kAcosfUlps).lo, widenF(acosf((float)z.lo), kAcosfUlps).hi};
   // atan2 over the box x * y: off the origin and the branch cut (x < 0, y = 0) its extremes are at the corners
   if (x.lo <= 0 && x.hi >= 0 && y.lo <= 0 && y.hi >= 0) return kUndecided;
+  // The cut: where y's interval holds 0 with x < 0.  A y that crosses 0 is also refused by the theta test below (the
+  // corners' atan2f have opposite signs); this test covers the ends that are zeros, whose sign the interval does not
+  // track while the host's atan2f(+-0, x < 0) = +-pi does
   if (x.lo < 0 && y.lo <= 0 && y.hi >= 0) return kUndecided;
   double tlo = INFINITY, thi = -INFINITY;
   for (int k = 0; k < 4; ++k) {

@@ -36,6 +36,25 @@
  *
  * derp_test_rig_*_host: the same computations on the host (DERP_HD code, the reference's loops), with host pointers,
  * for tests without a GPU.
+ *
+ * Probes of the device's interval proofs, for tests: each runs the device function the kernels run on the given inputs
+ * (host pointers in and out, on `device`).
+ * derp_test_math: the device's function fn (DERP_MATH_*) of a[i] (and b[i]; acosf and atan2f take them narrowed to
+ *   float): out[3 i] the value, out[3 i + 1 .. 3 i + 2] the interval the proofs widen it to (derp_interval.cuh's widenD
+ *   / widenF; the value itself for DERP_MATH_ATAN2POS, the sweep's FTHETA atan2).
+ * derp_test_acosf_exhaustive: every float x in [-1, 1], the device's acosf against the host's acosf and acos(double(x));
+ *   stats[0] and stats[1] the greatest device and host errors in ulps of acos(double(x)) times 2^20, stats[2] the
+ *   greatest distance between the two in float steps, stats[3] the host values outside the device value's widenF.
+ * derp_test_rig_point_iv: rigPointIv of cam's pixels (pix[2 i], pix[2 i + 1]) at depth: out[7 i .. 7 i + 5] the
+ *   intervals (lo, hi) of x, y and z, out[7 i + 6] undistort's result for the pixel.  Host twin: derp_test_camera_rig
+ *   at the pixel's centre.
+ * derp_test_sees_iv: seesIv of cam on the boxes boxes[6 i .. 6 i + 5] = (x lo, x hi, y lo, y hi, z lo, z hi):
+ *   decision[i] 1 (seen), 0 (not seen) or -1 (undecided), py[2 i .. 2 i + 1] the pixel row's interval when seen.  Host
+ *   twin: derp_test_camera_sees.
+ * derp_test_sees_device: the device's Camera::sees of exact points, as derp_test_camera_sees on the host.
+ * derp_test_proven_count: provenCount with timing of exact points: counts[i] the cameras that see point i and
+ *   timing[i] its minTimingDiff, or counts[i] = -1 where the device leaves the point to the host.
+ * derp_test_count_timing_host: the host twin (saveEquirect's per-point loop): counts[i] and timing[i] always.
  */
 #ifndef DERP_RIGANALYSIS_H_
 #define DERP_RIGANALYSIS_H_
@@ -66,6 +85,27 @@ int derp_test_rig_camera_coverage_host(const DerpCameraDesc* cams, const double*
                                        double distance, int32_t* counts);
 int derp_test_rig_cross_section_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, int dim,
                                      int32_t* counts);
+
+enum {
+  DERP_MATH_SIN = 0,
+  DERP_MATH_COS = 1,
+  DERP_MATH_ATAN = 2,
+  DERP_MATH_ASIN = 3,
+  DERP_MATH_ATAN2 = 4,
+  DERP_MATH_ACOSF = 5,
+  DERP_MATH_ATAN2F = 6,
+  DERP_MATH_ATAN2POS = 7
+};
+int derp_test_math(int device, int fn, const double* a, const double* b, int n, double* out);
+int derp_test_acosf_exhaustive(int device, uint32_t* stats);
+int derp_test_rig_point_iv(int device, const DerpCameraDesc* cam, const int32_t* pix, int n, double depth, double* out);
+int derp_test_sees_iv(int device, const DerpCameraDesc* cam, const double* boxes, int n, int32_t* decision,
+                      double* py);
+int derp_test_sees_device(int device, const DerpCameraDesc* cam, const double* pts, int n, double* pix, uint8_t* seen);
+int derp_test_proven_count(int device, const DerpCameraDesc* cams, const double* rotation9, int num_cams,
+                           const double* pts, int n, int32_t* counts, float* timing);
+int derp_test_count_timing_host(const DerpCameraDesc* cams, const double* rotation9, int num_cams, const double* pts,
+                                int n, int32_t* counts, float* timing);
 
 #ifdef __cplusplus
 }

@@ -30,6 +30,10 @@
  *   (derp_rigsim.cuh documents the bound).  derp_rigsim_last_host_rays: the number of rays the calling thread's last
  *   render resolved on the host (its share of derp_rigsim_last_rays, the supersample rays traced).
  *   derp_test_rigsim_area: the area kernel alone on src ([dh k][dw k][cn] floats) into dst ([dh][dw][cn]), for tests.
+ *   derp_test_sky_texel: a probe of the device's proof of the sky texel, for tests: skyTexelDevice of the directions
+ *     dirs[3 i .. 3 i + 2] of a rows x cols skybox into texel[2 i] (row) and texel[2 i + 1] (column), or (-1, -1) where
+ *     the device leaves the ray to the host; on `device` with host pointers.
+ *   derp_test_sky_texel_host: its host twin (the C library's acosf and atan2f), which always decides.
  *   derp_rigsim_trace_host: traceRayToGetColor (RigSimulator.cpp:196-262) on the host for n fp32 rays {origin, dir}:
  *     out[4 i .. 4 i + 3] = B, G, R (0..1), depth.  For tests without a GPU.
  */
@@ -100,6 +104,8 @@ uint64_t derp_rigsim_last_host_rays(void);
 uint64_t derp_rigsim_last_rays(void);
 
 int derp_test_rigsim_area(int device, const float* src, int dw, int dh, int cn, int k, float* dst);
+int derp_test_sky_texel(int device, const float* dirs, int n, int rows, int cols, int32_t* texel);
+int derp_test_sky_texel_host(const float* dirs, int n, int rows, int cols, int32_t* texel);
 int derp_rigsim_trace_host(const DerpRigsimScene* scene, const DerpRigsimRender* opts, const float* rays, int n,
                            float* out);
 

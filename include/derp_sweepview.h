@@ -55,6 +55,10 @@
  * the host.
  * derp_test_project_equirect_masks_host: the same per-pixel function on the host, with host pointers, for tests without a
  * GPU.
+ * derp_test_eqr_index_proven: a probe of the device's proof, for tests: the mask index (>= 0), -1 (nothing read) or -2
+ *   (undecided) that eqrIndexProven gives for the boxes boxes[6 i .. 6 i + 5] = (x lo, x hi, y lo, y hi, z lo, z hi) of
+ *   a width x height mask, on `device` with host pointers.
+ * derp_test_eqr_index_host: its host twin, eqrIndex of the points pts[3 i .. 3 i + 2]: the index or -1.
  */
 #ifndef DERP_SWEEPVIEW_H_
 #define DERP_SWEEPVIEW_H_
@@ -90,6 +94,8 @@ uint64_t derp_project_last_host_pixels(void);
 int derp_test_project_equirect_masks_host(const DerpCameraDesc* cams, int num_cams, double depth,
                                           const uint8_t* const* eqr_masks, const int32_t* mask_sizes,
                                           uint8_t* const* out);
+int derp_test_eqr_index_proven(int device, const double* boxes, int n, int width, int height, int64_t* out);
+int derp_test_eqr_index_host(const double* pts, int n, int width, int height, int64_t* out);
 
 #ifdef __cplusplus
 }
