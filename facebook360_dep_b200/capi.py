@@ -328,6 +328,31 @@ def _ptr_array(arrs):
     return pa
 
 
+# ---- include/derp_blur.h ------------------------------------------------------------------------------------------
+_BLUR_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_gaussian_blur": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+}
+BLUR_SYMBOLS = ["derp_gaussian_blur"]
+
+
+class Blur(_Binding):
+    """ctypes binding of include/derp_blur.h on a loaded library: ``Blur(load_cuda())``."""
+
+    def __init__(self, library):
+        self.path, self.lib = _bind(library, _BLUR_SIGS)
+
+    check = _Binding._check
+
+    def gaussian_blur(self, image, radius, device=0):
+        """cv::GaussianBlur((2 radius + 1)^2, sigma 0) of a u16 HxWx3 image (cv_util::gaussianBlur), radius 0 to 64."""
+        image = np.ascontiguousarray(image, np.uint16)
+        h, w = image.shape[:2]
+        out = np.empty((h, w, 3), np.uint16)
+        self.check(self.lib.derp_gaussian_blur(device, image.ctypes.data, w, h, radius, out.ctypes.data))
+        return out
+
+
 # ---- include/derp_rephoto.h ---------------------------------------------------------------------------------------
 _REPHOTO_SIGS = {
     "derp_last_error": (C.c_char_p, []),

@@ -11,6 +11,7 @@
 #include <map>
 #include <memory>
 
+#include "../../include/derp_blur.h"
 #include "derp_host.cuh"
 #include "derp_kernels.cuh"
 #include "derp_refine.cuh"
@@ -1288,6 +1289,72 @@ int derp_foreground_mask(int device, const uint16_t* templ, const uint16_t* fram
   CU(cudaGetLastError());
   CU(cudaMemcpy(mask, sc.dM.p, n, cudaMemcpyDefault));
   CU(cudaDeviceSynchronize());  // return with mask written, also when it is device memory (that copy does not wait)
+  return DERP_OK;
+}
+
+// The taps of cv::GaussianBlur((2 r + 1)^2, sigma 0) as OpenCV's bit-exact path builds them (getGaussianKernelBitExact,
+// then getGaussianKernelFixedPoint_ED with 16 fraction bits): its table kernels for sizes 3, 5, 7 and 9; above those the
+// sampled Gaussian with sigma = 0.15 n + 0.35 (one rounding), normalised to sum 1, scaled to 2^16 with error diffusion
+// over the left half and mirrored, the centre tap taking what is left of 2^16.
+static GaussTaps gaussTaps(int r) {
+  GaussTaps t{};
+  t.r = r;
+  const int n = 2 * r + 1;
+  if (r <= 4) {  // left halves and centres of {1 2 1} / 4, {1 4 6 4 1} / 16, {2 7 14 18 14 7 2} / 64, {4 13 30 51 60 ...} / 256
+    static const uint32_t kTable[5][5] = {{1}, {1, 2}, {1, 4, 6}, {2, 7, 14, 18}, {4, 13, 30, 51, 60}};
+    for (int i = 0; i <= r; ++i) t.k[i] = t.k[n - 1 - i] = kTable[r][i] << (16 - 2 * r);
+    return t;
+  }
+  const double sigma = std::fma((double)n, 0.15, 0.35), scale = -0.125 / (sigma * sigma);
+  double half[kGaussMaxRadius], sum = 0;
+  for (int i = 0, x = 1 - n; i < r; ++i, x += 2) {
+    half[i] = std::exp((double)(x * x) * scale);
+    sum += half[i];
+  }
+  const double mul = 1.0 / (sum * 2 + 1);
+  double err = 0;
+  uint32_t side = 0;
+  for (int i = 0; i < r; ++i) {
+    const double a = half[i] * mul * 65536.0 + err, v = std::nearbyint(a);  // cvRound: to nearest, ties to even
+    err = a - v;
+    t.k[i] = t.k[n - 1 - i] = (uint32_t)v;
+    side += (uint32_t)v;
+  }
+  t.k[r] = 65536u - 2 * side;
+  return t;
+}
+
+int derp_gaussian_blur(int device, const uint16_t* src, int width, int height, int radius, uint16_t* dst) {
+  if (!src || !dst || width < 1 || height < 1 || radius < 0 || radius > kGaussMaxRadius)
+    return fail(DERP_EINVAL, "derp_gaussian_blur: bad arguments (radius 0 to " + std::to_string(kGaussMaxRadius) + ")");
+  CU(cudaSetDevice(device));
+  const size_t n = (size_t)width * height * 3;
+  if (radius == 0) {  // a 1 x 1 kernel: a copy
+    if (src != dst) CU(cudaMemcpy(dst, src, n * sizeof(uint16_t), cudaMemcpyDefault));
+    CU(cudaDeviceSynchronize());  // also when both are device memory (that copy does not wait)
+    return DERP_OK;
+  }
+  // grow-only scratch per host thread: staged images and the row pass's u32 sums
+  static thread_local struct {
+    DevBuf<uint16_t> src, dst;
+    DevBuf<uint32_t> rows;
+  } sc;
+  const uint16_t* sp = src;
+  uint16_t* dp = dst;
+  int rc = stageIn(sp, n, sc.src);
+  if (rc || (rc = outBuffer(dp, n, sc.dst))) return rc;
+  CU(sc.rows.ensure(n));
+  const GaussTaps taps = gaussTaps(radius);
+  const dim3 rowGrid((width + kGaussRowPixels - 1) / kGaussRowPixels, std::min(height, 65535));
+  gaussRowKernel<<<rowGrid, 256, 3 * (kGaussRowPixels + 2 * radius) * sizeof(uint32_t)>>>(sp, width, height, taps,
+                                                                                          sc.rows.p);
+  const dim3 colGrid((unsigned)((3 * (size_t)width + kGaussColElems - 1) / kGaussColElems),
+                     (height + kGaussColRows - 1) / kGaussColRows);
+  gaussColKernel<<<colGrid, dim3(kGaussColElems, kGaussColThreadsY),
+                   (kGaussColRows + 2 * radius) * kGaussColElems * sizeof(uint32_t)>>>(sc.rows.p, width, height, taps, dp);
+  CU(cudaGetLastError());
+  if ((rc = stageOut(dst, dp, n))) return rc;
+  CU(cudaDeviceSynchronize());  // return with dst written, also when it is device memory
   return DERP_OK;
 }
 

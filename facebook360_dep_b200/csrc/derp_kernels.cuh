@@ -1129,6 +1129,66 @@ __global__ void gaussian3Kernel(const uint16_t* __restrict__ src, int w, int h, 
     for (int i = 0; i < 3; ++i) s += (unsigned)((j == 1 ? 2 : 1) * (i == 1 ? 2 : 1)) * src[((size_t)ys[j] * w + xs[i]) * 3 + c];
   dst[((size_t)y * w + x) * 3 + c] = (uint16_t)((s + 8u) >> 4);
 }
+// cv::GaussianBlur((2 r + 1)^2, sigma 0) on u16 x 3 for any radius up to kGaussMaxRadius (derp_gaussian_blur): OpenCV's
+// bit-exact fixed-point path.  Taps carry 16 fraction bits and sum to 2^16 (built on the host, gaussTaps in derp_b200.cu).
+// The row pass keeps exact u32 sums (at most 65535 * 2^16); the column pass sums those in u64 and rounds with
+// (s + 2^31) >> 32.  Borders are REFLECT_101, folded as often as an image smaller than the kernel needs.
+constexpr int kGaussMaxRadius = 64;
+struct GaussTaps {
+  int r;
+  uint32_t k[2 * kGaussMaxRadius + 1];  // k[r - i] == k[r + i]
+};
+__device__ __forceinline__ int reflect101Fold(int p, int len) {  // == reflect101, in closed form: period 2 (len - 1)
+  if (len == 1) return 0;
+  const int period = 2 * (len - 1);
+  p = abs(p) % period;
+  return p < len ? p : period - p;
+}
+// Row pass: one block per kGaussRowPixels pixels of a row; the row segment and its aprons are staged in shared memory as
+// u32 elements (interleaved like the image, so consecutive threads read consecutive words)
+constexpr int kGaussRowPixels = 256;
+__global__ void __launch_bounds__(256) gaussRowKernel(const uint16_t* __restrict__ src, int w, int h, GaussTaps t,
+                                                      uint32_t* __restrict__ rows) {
+  extern __shared__ uint32_t sRow[];
+  const int r = t.r, x0 = blockIdx.x * kGaussRowPixels;
+  const int px = min(kGaussRowPixels, w - x0), ne = 3 * (px + 2 * r);
+  for (int y = blockIdx.y; y < h; y += gridDim.y) {  // the grid's y extent is capped at 65535 rows
+    const uint16_t* S = src + (size_t)y * w * 3;
+    for (int e = threadIdx.x; e < ne; e += blockDim.x) {
+      const int p = e / 3, c = e - 3 * p;
+      sRow[e] = S[reflect101Fold(x0 - r + p, w) * 3 + c];
+    }
+    __syncthreads();
+    uint32_t* D = rows + ((size_t)y * w + x0) * 3;
+    for (int e = threadIdx.x; e < 3 * px; e += blockDim.x) {
+      const uint32_t* s = sRow + e + 3 * r;  // the output element's own tap
+      uint32_t sum = t.k[r] * s[0];
+      for (int i = 1; i <= r; ++i) sum += t.k[r - i] * (s[-3 * i] + s[3 * i]);  // < 2^32: the taps sum to 2^16
+      D[e] = sum;
+    }
+    __syncthreads();
+  }
+}
+// Column pass: a block covers kGaussColElems elements of kGaussColRows output rows and stages the rows it reads
+constexpr int kGaussColElems = 32, kGaussColRows = 64, kGaussColThreadsY = 8;
+__global__ void __launch_bounds__(kGaussColElems* kGaussColThreadsY) gaussColKernel(const uint32_t* __restrict__ rows, int w,
+                                                                                   int h, GaussTaps t,
+                                                                                   uint16_t* __restrict__ dst) {
+  extern __shared__ uint32_t sCol[];
+  const int r = t.r, n = 3 * w, tx = threadIdx.x;
+  const int e = blockIdx.x * kGaussColElems + tx, y0 = blockIdx.y * kGaussColRows;
+  const int ny = min(kGaussColRows, h - y0), nr = ny + 2 * r;
+  for (int j = threadIdx.y; j < nr; j += kGaussColThreadsY)
+    sCol[j * kGaussColElems + tx] = e < n ? rows[(size_t)reflect101Fold(y0 - r + j, h) * n + e] : 0u;
+  __syncthreads();
+  if (e >= n) return;
+  for (int j = threadIdx.y; j < ny; j += kGaussColThreadsY) {
+    const uint32_t* s = sCol + j * kGaussColElems + tx;
+    unsigned long long sum = 0;
+    for (int i = 0; i <= 2 * r; ++i) sum += (unsigned long long)t.k[i] * s[i * kGaussColElems];
+    dst[(size_t)(y0 + j) * n + e] = (uint16_t)((sum + (1ull << 31)) >> 32);
+  }
+}
 // mask = || float(template) - float(frame) ||_2 > threshold; cv::norm accumulates the squares in double
 __global__ void foregroundDiffKernel(size_t n, const uint16_t* __restrict__ templ, const uint16_t* __restrict__ frame, float threshold,
                                      uint8_t* __restrict__ mask) {

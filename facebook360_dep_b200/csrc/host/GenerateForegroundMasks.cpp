@@ -4,6 +4,7 @@
 // morphological closing: BackgroundSubtractionUtil.h:20-59) runs in libderp_b200.so.
 #include <thread>
 
+#include "../../../include/derp_blur.h"
 #include "io.h"
 
 const std::string kUsage = R"(
@@ -64,6 +65,7 @@ int main(int argc, char** argv) {
   CHECK_NE(FLAGS_background_frame, "");
   CHECK_GT(FLAGS_width, 0);
   CHECK_GE(FLAGS_blur_radius, 0);
+  CHECK_LE(FLAGS_blur_radius, 64) << "--blur_radius above 64 is not supported";
   CHECK_GE(FLAGS_threshold, 0);
   CHECK_GE(FLAGS_morph_closing_size, 0);
   const io::Rig rig = io::loadRig(FLAGS_rig);
@@ -80,13 +82,13 @@ int main(int argc, char** argv) {
   const int W = std::min(bw, FLAGS_width);
   const int H = (int)std::lrint(W * bh / float(bw));
   std::vector<std::vector<uint16_t>> background(cams.size());
-  // The library blurs with the default radius (1: its 3 x 3 kernel) or not at all; the UI's slider can ask for more: radii 2
-  // and 3 are blurred on the host (OpenCV's 5- and 7-tap table kernels, io.h) and the library is told not to blur.
-  const bool hostBlur = FLAGS_blur_radius > 1;
-  const int libraryBlur = hostBlur ? 0 : FLAGS_blur_radius;
+  // derp_foreground_mask blurs with the default radius (1: its 3 x 3 kernel) or not at all. Larger radii (the UI's slider
+  // goes up to 20) blur each background once and each frame with derp_gaussian_blur, and the mask is told not to blur.
+  const bool ownBlur = FLAGS_blur_radius > 1;
+  const int maskBlur = ownBlur ? 0 : FLAGS_blur_radius;
   for (size_t i = 0; i < cams.size(); ++i) {
     background[i] = loadResized(io::imagePath(FLAGS_background_color, rig.ids[cams[i]], FLAGS_background_frame), W, H, FLAGS_gpu);
-    if (hostBlur) background[i] = io::gaussianBlurU16C3(background[i], W, H, FLAGS_blur_radius);
+    if (ownBlur) DERP_CALL(derp_gaussian_blur(FLAGS_gpu, background[i].data(), W, H, FLAGS_blur_radius, background[i].data()));
   }
   for (int c : cams) fs::create_directories(fs::path(FLAGS_foreground_masks) / rig.ids[c]);
 
@@ -109,9 +111,9 @@ int main(int argc, char** argv) {
         for (size_t k = 0; k < cams.size(); ++k) {
           const std::string& id = rig.ids[cams[k]];
           std::vector<uint16_t> color = loadResized(io::imagePath(FLAGS_color, id, frame), W, H, device);
-          if (hostBlur) color = io::gaussianBlurU16C3(color, W, H, FLAGS_blur_radius);
+          if (ownBlur) DERP_CALL(derp_gaussian_blur(device, color.data(), W, H, FLAGS_blur_radius, color.data()));
           std::vector<uint8_t> mask((size_t)W * H);
-          DERP_CALL(derp_foreground_mask(device, background[k].data(), color.data(), W, H, libraryBlur,
+          DERP_CALL(derp_foreground_mask(device, background[k].data(), color.data(), W, H, maskBlur,
                                          (float)FLAGS_threshold, FLAGS_morph_closing_size, mask.data()));
           size_t count = 0;
           for (uint8_t& m : mask) {

@@ -778,8 +778,8 @@ inline std::vector<uint8_t> loadRgba8(const fs::path& path, int* w, int* h) {
 // cv_util::gaussianBlur(image, radius) = cv::GaussianBlur(image, (2 r + 1)^2, sigma 0) (CvUtil.h:302-312) on a 16-bit
 // 3-channel image, radius 1..3: OpenCV's fixed-point path with its table kernels for sizes up to 7 — (1 2 1) / 4,
 // (1 4 6 4 1) / 16, (2 7 14 18 14 7 2) / 64 — i.e. the integer-weighted sum, + half, shifted; BORDER_REFLECT_101 (pinned to
-// cv2 in tests/test_apps.py).  The CUDA library blurs with the default radius 1 itself (derp_foreground_mask); the larger
-// radii of the UI's slider are blurred here and handed over with blur_radius = 0.
+// cv2 in tests/test_apps.py).  GenerateForegroundMasks blurs with the library at every radius (derp_foreground_mask,
+// derp_gaussian_blur); this host restatement stays as IoSelfTest --mode=gauss's reference for the table kernels.
 inline std::vector<uint16_t> gaussianBlurU16C3(const std::vector<uint16_t>& src, int w, int h, int radius) {
   CHECK(radius >= 1 && radius <= 3) << "--blur_radius up to 3 (OpenCV's table kernels); got " << radius;
   static const int kernels[3][7] = {{1, 2, 1}, {1, 4, 6, 4, 1}, {2, 7, 14, 18, 14, 7, 2}};
