@@ -1659,6 +1659,11 @@ int derp_joint_bilateral_f32(int device, int width, int height, const float* ima
 // ---- host-side test hooks ---------------------------------------------------------------------------
 // The selection, RNG and camera code is __host__ __device__; these entry points run the HOST
 // instantiation so that CPU-only tests (-m "not gpu") can check it against libstdc++ / the oracle.
+static __global__ void appendRangeKernel(int n, UndecidedView<unsigned long long> undecided) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) undecided.append(i);
+}
+
 extern "C" {
 
 // 1 if the three-instruction constant division (derp_divconst.cuh) was validated exact for divisor c on `device`
@@ -1668,6 +1673,24 @@ int derp_test_div_const(int device, float c) {
   DivConst k;
   if (makeDivConst(c, 0, &k) != cudaSuccess) return DERP_ECUDA;
   return k.fast;
+}
+
+// UndecidedList::collect (derp_host.cuh) on a kernel that appends 0 .. n - 1, from a new list of start_capacity
+// entries: the n items in list order into out; returns the number of launches it took, < 0 on error.
+int derp_test_undecided_list(int device, int n, uint64_t start_capacity, uint64_t* out) {
+  if (n < 0 || start_capacity < 1 || !out) return fail(DERP_EINVAL, "derp_test_undecided_list: bad arguments");
+  CU(cudaSetDevice(device));
+  UndecidedList<unsigned long long> list;
+  std::vector<unsigned long long> items;
+  int launches = 0;
+  auto launch = [&](UndecidedView<unsigned long long> undecided) {
+    ++launches;
+    appendRangeKernel<<<grid1(std::max(n, 1)), 256>>>(n, undecided);
+    return DERP_OK;
+  };
+  if (int rc = list.collect(launch, items, start_capacity)) return rc;
+  std::copy(items.begin(), items.end(), out);
+  return launches;
 }
 
 // Host instantiation of the table-driven selection (derp_select.cuh): returns 1 and the sum when the table path

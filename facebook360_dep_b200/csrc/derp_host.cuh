@@ -1,5 +1,5 @@
-// Host-side plumbing shared by the library's translation units: the error string, device buffers, launch shapes and
-// the one rule that decides whether a kernel may use a caller's pointer in place.
+// Host-side plumbing shared by the library's translation units: the error string, device buffers, launch shapes, the one
+// rule that decides whether a kernel may use a caller's pointer in place, and the interval proofs' undecided list.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -138,6 +138,48 @@ int stageOut(T* dst, const T* written, size_t count) {
   if (written != dst) CU(cudaMemcpy(dst, written, count * sizeof(T), cudaMemcpyDefault));
   return DERP_OK;
 }
+
+// ---- undecided lists ----------------------------------------------------------------------------------------------
+// A kernel that proves the reference's decisions appends each item its proof leaves open through an UndecidedView
+// (passed by value); the host decides those items with the DERP_HD code and the C library.  append counts every item
+// and stores those below the capacity, so a count above it tells the host how large the list must be.
+template <typename T>
+struct UndecidedView {
+  T* items;
+  unsigned long long capacity;
+  unsigned long long* count;
+  __device__ __forceinline__ void append(const T& item) const {
+    const unsigned long long slot = atomicAdd(count, 1ull);
+    if (slot < capacity) items[slot] = item;
+  }
+};
+
+// A list's grow-only device buffers, 2^20 entries at first; after collect() `items` holds the list for the caller's
+// resolve kernel.  collect calls launch(view) (DERP_OK or an error code) and, when the count exceeded the capacity,
+// relaunches it with a list of that size: the kernels' decisions are deterministic, so it lists the same items.  out
+// receives the items in list order.
+template <typename T>
+struct UndecidedList {
+  DevBuf<T> items;
+  DevBuf<unsigned long long> count;
+  template <class Launch>
+  int collect(Launch launch, std::vector<T>& out, unsigned long long capacity = 1ull << 20) {
+    CU(count.ensure(1));
+    CU(items.ensure(capacity));
+    unsigned long long n = 0;
+    for (;;) {
+      CU(cudaMemset(count.p, 0, sizeof n));
+      if (int rc = launch(UndecidedView<T>{items.p, (unsigned long long)items.n, count.p})) return rc;
+      CU(cudaGetLastError());
+      CU(cudaMemcpy(&n, count.p, sizeof n, cudaMemcpyDeviceToHost));
+      if (n <= items.n) break;
+      CU(items.ensure(n));
+    }
+    out.resize(n);
+    if (n) CU(cudaMemcpy(out.data(), items.p, n * sizeof(T), cudaMemcpyDeviceToHost));
+    return DERP_OK;
+  }
+};
 
 // Enables the current device's direct access to `other`'s memory where the two have a peer path (NVLink)
 inline int enablePeer(int device, int other) {

@@ -16,21 +16,14 @@ namespace {
 struct RigScratch {
   DevBuf<DevCamera> cams;
   DevBuf<double> tabs;
-  DevBuf<unsigned long long> hist, undecided, count;
+  DevBuf<unsigned long long> hist;
+  UndecidedList<unsigned long long> undecided;  // pixel index, or distance << 32 | sample for the histogram
   DevBuf<int32_t> counts, resolvedCounts;
   DevBuf<float> timing, resolvedTiming;
 };
 thread_local RigScratch g_rigA;
 thread_local unsigned long long g_rigHostPoints = 0;  // points the last call resolved on the host
-constexpr unsigned long long kUndecidedCapacity = 1ull << 16;  // list entries kept between calls (grown on demand)
 constexpr int kThreads = 256;
-
-// Lists point `index` for the host
-__device__ __forceinline__ void listPoint(unsigned long long index, unsigned long long* list, unsigned long long cap,
-                                          unsigned long long* count) {
-  const unsigned long long slot = atomicAdd(count, 1ull);
-  if (slot < cap) list[slot] = index;
-}
 
 // main's coverage loop: thread (j, k) counts the cameras that see distances[k] * samples[j] into hist[k][count]; one
 // atomic per distinct count in the warp
@@ -38,13 +31,12 @@ __global__ void __launch_bounds__(kThreads) coverageKernel(const DevCamera* __re
                                                            const double* __restrict__ samples, int numSamples,
                                                            const double* __restrict__ distances,
                                                            unsigned long long* __restrict__ hist,
-                                                           unsigned long long* list, unsigned long long cap,
-                                                           unsigned long long* count) {
+                                                           UndecidedView<unsigned long long> undecided) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x, k = blockIdx.y;
   if (j >= numSamples) return;
   const double d = distances[k];
   const int c = provenCount<false>(cams, n, d * samples[3 * j], d * samples[3 * j + 1], d * samples[3 * j + 2], nullptr);
-  if (c < 0) listPoint((unsigned long long)k << 32 | (unsigned)j, list, cap, count);
+  if (c < 0) undecided.append((unsigned long long)k << 32 | (unsigned)j);
   const unsigned peers = __match_any_sync(__activemask(), c);
   if (c >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1)
     atomicAdd(&hist[(size_t)k * (n + 1) + c], (unsigned long long)__popc(peers));
@@ -55,8 +47,7 @@ __global__ void __launch_bounds__(kThreads) coverageKernel(const DevCamera* __re
 __global__ void __launch_bounds__(kThreads) equirectKernel(const DevCamera* __restrict__ cams, int n, int W, int H,
                                                            const double* __restrict__ tabs, double distance,
                                                            int32_t* __restrict__ counts, float* __restrict__ timing,
-                                                           unsigned long long* list, unsigned long long cap,
-                                                           unsigned long long* count) {
+                                                           UndecidedView<unsigned long long> undecided) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= W) return;
   const double cl = tabs[y], sl = tabs[H + y], co = tabs[2 * H + x], so = tabs[2 * H + W + x];
@@ -64,7 +55,7 @@ __global__ void __launch_bounds__(kThreads) equirectKernel(const DevCamera* __re
   const size_t at = (size_t)y * W + x;
   float m = 1.0f;
   const int c = timing ? provenCount<true>(cams, n, px, py, pz, &m) : provenCount<false>(cams, n, px, py, pz, nullptr);
-  if (c < 0) listPoint(at, list, cap, count);
+  if (c < 0) undecided.append(at);
   counts[at] = c;
   if (timing) timing[at] = m;
 }
@@ -73,8 +64,8 @@ __global__ void __launch_bounds__(kThreads) equirectKernel(const DevCamera* __re
 // see the interval of cam.rig({x + .5, y + .5}, distance)
 __global__ void __launch_bounds__(kThreads) cameraKernel(const DevCamera* __restrict__ cams, int n, int cam,
                                                          double edge2, int W, int H, double distance,
-                                                         int32_t* __restrict__ counts, unsigned long long* list,
-                                                         unsigned long long cap, unsigned long long* count) {
+                                                         int32_t* __restrict__ counts,
+                                                         UndecidedView<unsigned long long> undecided) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= W) return;
   const size_t at = (size_t)y * W + x;
@@ -94,7 +85,7 @@ __global__ void __launch_bounds__(kThreads) cameraKernel(const DevCamera* __rest
     const int s = seesIv(cams[i], w, &py);
     if (s == kUndecided) {
       total = -1;
-      listPoint(at, list, cap, count);
+      undecided.append(at);
       break;
     }
     total += s;
@@ -104,13 +95,13 @@ __global__ void __launch_bounds__(kThreads) cameraKernel(const DevCamera* __rest
 
 // saveCrossSection's point (x + .5 - .5 dim, y + .5 - .5 dim, 0), exact
 __global__ void __launch_bounds__(kThreads) crossSectionKernel(const DevCamera* __restrict__ cams, int n, int dim,
-                                                               int32_t* __restrict__ counts, unsigned long long* list,
-                                                               unsigned long long cap, unsigned long long* count) {
+                                                               int32_t* __restrict__ counts,
+                                                               UndecidedView<unsigned long long> undecided) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= dim) return;
   const size_t at = (size_t)y * dim + x;
   const int c = provenCount<false>(cams, n, x + 0.5 - 0.5 * dim, y + 0.5 - 0.5 * dim, 0.0, nullptr);
-  if (c < 0) listPoint(at, list, cap, count);
+  if (c < 0) undecided.append(at);
   counts[at] = c;
 }
 
@@ -157,28 +148,6 @@ std::vector<double> equirectTables(int W, int H) {
   return t;
 }
 
-// Launches `run(list, cap, count)` until the undecided list holds every listed point (the decisions are deterministic,
-// so a second launch lists the same points) and returns the list in host memory
-template <class Run>
-int runListed(Run run, std::vector<unsigned long long>& list) {
-  RigScratch& g = g_rigA;
-  CU(g.count.ensure(1));
-  CU(g.undecided.ensure(kUndecidedCapacity));
-  unsigned long long count = 0;
-  for (;;) {
-    CU(cudaMemset(g.count.p, 0, sizeof count));
-    if (int rc = run(g.undecided.p, (unsigned long long)g.undecided.n, g.count.p)) return rc;
-    CU(cudaGetLastError());
-    CU(cudaMemcpy(&count, g.count.p, sizeof count, cudaMemcpyDeviceToHost));
-    if (count <= g.undecided.n) break;
-    CU(g.undecided.ensure(count));
-  }
-  list.resize(count);
-  if (count) CU(cudaMemcpy(list.data(), g.undecided.p, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  g_rigHostPoints = count;
-  return DERP_OK;
-}
-
 // Writes the host's values c (and t) of the listed pixels into the device planes
 int resolvePixels(const std::vector<unsigned long long>& list, const std::vector<int32_t>& c,
                   const std::vector<float>* t, int32_t* counts, float* timing) {
@@ -187,8 +156,8 @@ int resolvePixels(const std::vector<unsigned long long>& list, const std::vector
   if (int rc = upload(g.resolvedCounts, c.data(), c.size())) return rc;
   if (t)
     if (int rc = upload(g.resolvedTiming, t->data(), t->size())) return rc;
-  resolveKernel<<<grid1(list.size()), 256>>>(g.undecided.p, g.resolvedCounts.p, t ? g.resolvedTiming.p : nullptr,
-                                             (int)list.size(), counts, timing);
+  resolveKernel<<<grid1(list.size()), 256>>>(g.undecided.items.p, g.resolvedCounts.p,
+                                             t ? g.resolvedTiming.p : nullptr, (int)list.size(), counts, timing);
   CU(cudaGetLastError());
   return DERP_OK;
 }
@@ -338,12 +307,13 @@ int derp_rig_coverage(int device, const DerpCameraDesc* cams, const double* rota
   CU(cudaMemset(g.hist.p, 0, nh * sizeof(unsigned long long)));
   std::vector<unsigned long long> list;
   const dim3 grid(grid1(num_samples, kThreads), num_distances);
-  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
+  auto run = [&](UndecidedView<unsigned long long> undecided) {
     CU(cudaMemset(g.hist.p, 0, nh * sizeof(unsigned long long)));
-    coverageKernel<<<grid, kThreads>>>(g.cams.p, num_cams, g.tabs.p, num_samples, dist.p, g.hist.p, l, cap, count);
+    coverageKernel<<<grid, kThreads>>>(g.cams.p, num_cams, g.tabs.p, num_samples, dist.p, g.hist.p, undecided);
     return DERP_OK;
   };
-  if (int rc = runListed(run, list)) return rc;
+  if (int rc = g.undecided.collect(run, list)) return rc;
+  g_rigHostPoints = list.size();
   std::vector<unsigned long long> h(nh);
   CU(cudaMemcpy(h.data(), g.hist.p, nh * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   for (unsigned long long e : list) {
@@ -376,11 +346,12 @@ int derp_rig_equirect_coverage(int device, const DerpCameraDesc* cams, const dou
     if (int rc = outBuffer(dt, np, g.timing)) return rc;
   std::vector<unsigned long long> list;
   const dim3 grid(grid1(width, kThreads), height);
-  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
-    equirectKernel<<<grid, kThreads>>>(g.cams.p, num_cams, width, height, g.tabs.p, distance, dc, dt, l, cap, count);
+  auto run = [&](UndecidedView<unsigned long long> undecided) {
+    equirectKernel<<<grid, kThreads>>>(g.cams.p, num_cams, width, height, g.tabs.p, distance, dc, dt, undecided);
     return DERP_OK;
   };
-  if (int rc = runListed(run, list)) return rc;
+  if (int rc = g.undecided.collect(run, list)) return rc;
+  g_rigHostPoints = list.size();
   std::vector<int32_t> rc(list.size());
   std::vector<float> rt(list.size()), scratch(num_cams);
   for (size_t k = 0; k < list.size(); ++k) {
@@ -414,11 +385,12 @@ int derp_rig_camera_coverage(int device, const DerpCameraDesc* cams, const doubl
   if (int rc = outBuffer(dc, np, g.counts)) return rc;
   std::vector<unsigned long long> list;
   const dim3 grid(grid1(W, kThreads), H);
-  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
-    cameraKernel<<<grid, kThreads>>>(g.cams.p, num_cams, cam, edge2, W, H, distance, dc, l, cap, count);
+  auto run = [&](UndecidedView<unsigned long long> undecided) {
+    cameraKernel<<<grid, kThreads>>>(g.cams.p, num_cams, cam, edge2, W, H, distance, dc, undecided);
     return DERP_OK;
   };
-  if (int rc = runListed(run, list)) return rc;
+  if (int rc = g.undecided.collect(run, list)) return rc;
+  g_rigHostPoints = list.size();
   std::vector<int32_t> rc(list.size());
   for (size_t k = 0; k < list.size(); ++k)
     rc[k] = countCameraPixel(c.data(), num_cams, cam, edge2, (int)(list[k] % W), (int)(list[k] / W), distance);
@@ -441,11 +413,12 @@ int derp_rig_cross_section(int device, const DerpCameraDesc* cams, const double*
   if (int rc = outBuffer(dc, np, g.counts)) return rc;
   std::vector<unsigned long long> list;
   const dim3 grid(grid1(dim, kThreads), dim);
-  auto run = [&](unsigned long long* l, unsigned long long cap, unsigned long long* count) {
-    crossSectionKernel<<<grid, kThreads>>>(g.cams.p, num_cams, dim, dc, l, cap, count);
+  auto run = [&](UndecidedView<unsigned long long> undecided) {
+    crossSectionKernel<<<grid, kThreads>>>(g.cams.p, num_cams, dim, dc, undecided);
     return DERP_OK;
   };
-  if (int rc = runListed(run, list)) return rc;
+  if (int rc = g.undecided.collect(run, list)) return rc;
+  g_rigHostPoints = list.size();
   std::vector<int32_t> rc(list.size());
   for (size_t k = 0; k < list.size(); ++k)
     rc[k] = countSees(c.data(), num_cams, (int)(list[k] % dim) + 0.5 - 0.5 * dim, (int)(list[k] / dim) + 0.5 - 0.5 * dim,

@@ -28,14 +28,12 @@ struct RigsimScratch {
   DevBuf<DerpRigsimTriangle> tris;
   DevBuf<uint8_t> sky, ceil;
   DevBuf<float> bgrSS, p2SS, out0, out1, tables;
-  DevBuf<SkyRay> undecided;
+  UndecidedList<SkyRay> undecided;
   DevBuf<int2> texels;
-  DevBuf<unsigned long long> count;
   DevBuf<DevCamera> cam;
 };
 thread_local RigsimScratch g_rig;
 thread_local unsigned long long g_rigHostRays = 0, g_rigRays = 0;
-constexpr size_t kUndecidedCapacity = 1u << 16;  // list entries kept between calls (grown on demand)
 
 // One supersample's result into the supersampled planes: 255 * BGR and the second plane
 __device__ __forceinline__ void store(const float* c, size_t at, float* bgr, float* p2, int plane2) {
@@ -52,13 +50,12 @@ __device__ __forceinline__ void store(const float* c, size_t at, float* bgr, flo
 
 // The rest of traceRayToGetColor on the device: the sky texel when the interval proves it, else the ray is listed
 __device__ __forceinline__ void shadeRay(const SceneView& s, V3 o, V3 d, size_t at, float* bgr, float* p2, int plane2,
-                                         SkyRay* list, unsigned long long cap, unsigned long long* count) {
+                                         UndecidedView<SkyRay> undecided) {
   float c[4];
   if (!traceRay(s, o, d, c)) {
     int row, col;
     if (!skyTexelDevice(d, s.skyH, s.skyW, &row, &col)) {
-      const unsigned long long k = atomicAdd(count, 1ull);
-      if (k < cap) list[k] = SkyRay{(unsigned)at, {d.x, d.y, d.z}};
+      undecided.append(SkyRay{(unsigned)at, {d.x, d.y, d.z}});
       return;
     }
     skyColor(s, row, col, c);
@@ -70,7 +67,7 @@ __device__ __forceinline__ void shadeRay(const SceneView& s, V3 o, V3 d, size_t 
 // outside the image circle (0, 0, 0, FLT_MAX), else cam.rig(pixel) narrowed to fp32 and traced
 __global__ void __launch_bounds__(kTraceThreadsX* kTraceThreadsY)
     traceCameraKernel(SceneView s, const DevCamera* __restrict__ cam, int W, int H, int aas, float* bgr, float* depth,
-                      SkyRay* list, unsigned long long cap, unsigned long long* count) {
+                      UndecidedView<SkyRay> undecided) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= W || y >= H) return;
   const DevCamera& c = *cam;
@@ -84,7 +81,7 @@ __global__ void __launch_bounds__(kTraceThreadsX* kTraceThreadsY)
   double dir[3];
   pixelRay(c, px, py, dir);
   shadeRay(s, v3((float)c.pos[0], (float)c.pos[1], (float)c.pos[2]), v3((float)dir[0], (float)dir[1], (float)dir[2]),
-           at, bgr, depth, kDepth, list, cap, count);
+           at, bgr, depth, kDepth, undecided);
 }
 
 // renderMonoEquirect / renderStereoEquirect's supersamples (RigSimulator.cpp:529-545, 558-585): the direction
@@ -92,13 +89,12 @@ __global__ void __launch_bounds__(kTraceThreadsX* kTraceThreadsY)
 // origin 0 (mono) or the column's eye (stereo)
 __global__ void __launch_bounds__(kTraceThreadsX* kTraceThreadsY)
     traceEquirectKernel(SceneView s, int W, int H, const float* __restrict__ tab, const float* __restrict__ eyes,
-                        float* bgr, float* p2, int plane2, SkyRay* list, unsigned long long cap,
-                        unsigned long long* count) {
+                        float* bgr, float* p2, int plane2, UndecidedView<SkyRay> undecided) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= W || y >= H) return;
   const float sinP = tab[y], cosP = tab[H + y], cosT = tab[2 * H + x], sinT = tab[2 * H + W + x];
   const V3 o = eyes ? v3(eyes + 3 * x) : v3(0.0f, 0.0f, 0.0f);
-  shadeRay(s, o, v3(sinP * cosT, sinP * sinT, cosP), (size_t)y * W + x, bgr, p2, plane2, list, cap, count);
+  shadeRay(s, o, v3(sinP * cosT, sinP * sinT, cosP), (size_t)y * W + x, bgr, p2, plane2, undecided);
 }
 
 // The listed supersamples, with the texels the host found
@@ -191,21 +187,11 @@ int uploadScene(const DerpRigsimScene* sc, const DerpRigsimRender* o, SceneView&
 template <class Launch>
 int traceAndResolve(const SceneView& v, Launch trace, float* bgr, float* p2, int plane2, unsigned long long* hostRays) {
   RigsimScratch& g = g_rig;
-  CU(g.count.ensure(1));
-  CU(g.undecided.ensure(kUndecidedCapacity));
-  unsigned long long count = 0;
-  for (;;) {  // a second launch only when the list overflowed (the trace is deterministic)
-    CU(cudaMemset(g.count.p, 0, sizeof(unsigned long long)));
-    trace(g.undecided.p, (unsigned long long)g.undecided.n, g.count.p);
-    CU(cudaGetLastError());
-    CU(cudaMemcpy(&count, g.count.p, sizeof count, cudaMemcpyDeviceToHost));
-    if (count <= g.undecided.n) break;
-    CU(g.undecided.ensure(count));
-  }
+  std::vector<SkyRay> list;
+  if (int rc = g.undecided.collect(trace, list)) return rc;
+  const size_t count = list.size();
   *hostRays += count;
   if (!count) return DERP_OK;
-  std::vector<SkyRay> list(count);
-  CU(cudaMemcpy(list.data(), g.undecided.p, count * sizeof(SkyRay), cudaMemcpyDeviceToHost));
   std::vector<int2> tex(count);
   for (size_t k = 0; k < count; ++k) {
     int row, col;
@@ -213,7 +199,7 @@ int traceAndResolve(const SceneView& v, Launch trace, float* bgr, float* p2, int
     tex[k] = make_int2(row, col);
   }
   if (int rc = upload(g.texels, tex.data(), count)) return rc;
-  resolveSkyKernel<<<grid1(count), 256>>>(v, g.undecided.p, g.texels.p, (int)count, bgr, p2, plane2);
+  resolveSkyKernel<<<grid1(count), 256>>>(v, g.undecided.items.p, g.texels.p, (int)count, bgr, p2, plane2);
   CU(cudaGetLastError());
   return DERP_OK;
 }
@@ -312,8 +298,9 @@ int derp_rigsim_render_cameras(int device, const DerpRigsimScene* scene, const D
     const dim3 block(kTraceThreadsX, kTraceThreadsY), grid((W + block.x - 1) / block.x, (H + block.y - 1) / block.y);
     const DevCamera* cam = g.cam.p;
     float *b = g.bgrSS.p, *d = g.p2SS.p;
-    auto trace = [&](SkyRay* list, unsigned long long cap, unsigned long long* count) {
-      traceCameraKernel<<<grid, block>>>(v, cam, W, H, aas, b, d, list, cap, count);
+    auto trace = [&](UndecidedView<SkyRay> undecided) {
+      traceCameraKernel<<<grid, block>>>(v, cam, W, H, aas, b, d, undecided);
+      return DERP_OK;
     };
     if (int rc = traceAndResolve(v, trace, b, d, kDepth, &hostRays)) return rc;
     rays += n;
@@ -381,8 +368,9 @@ int derp_rigsim_render_equirect(int device, const DerpRigsimScene* scene, const 
     const int plane2 = stereo ? kNone : kInvDepth;
     const float* tabs = g.tables.p;
     const float* eye = stereo ? g.tables.p + nt + 3 * (size_t)W * e : nullptr;
-    auto trace = [&](SkyRay* list, unsigned long long cap, unsigned long long* count) {
-      traceEquirectKernel<<<grid, block>>>(v, W, H, tabs, eye, b, p2, plane2, list, cap, count);
+    auto trace = [&](UndecidedView<SkyRay> undecided) {
+      traceEquirectKernel<<<grid, block>>>(v, W, H, tabs, eye, b, p2, plane2, undecided);
+      return DERP_OK;
     };
     if (int rc = traceAndResolve(v, trace, b, p2, plane2, &hostRays)) return rc;
   }

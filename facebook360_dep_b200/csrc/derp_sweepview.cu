@@ -22,13 +22,12 @@ struct SweepScratch {
   DevBuf<uint8_t> maskUpload, maskOut;
   DevBuf<derp::sweep::EqrMask> masks;
   DevBuf<uint8_t*> maskOuts;
-  DevBuf<unsigned long long> undecided;
+  UndecidedList<unsigned long long> undecided;  // camera << 32 | pixel
   DevBuf<long long> resolved;
 };
 thread_local SweepScratch g_sweep;
 thread_local unsigned long long g_sweepHits = 0;  // contributing (sample, camera) pairs of the last call
 thread_local unsigned long long g_projectHostPixels = 0;  // pixels the last derp_project_equirect_masks left to the host
-constexpr unsigned long long kUndecidedCapacity = 1ull << 20;  // list entries kept between calls (grown on demand)
 
 // Cameras as the apps hold them (already rescaled), optionally centred on camera `center`
 int sweepCameras(const char* who, const DerpCameraDesc* cams, int n, int center, std::vector<DevCamera>& out) {
@@ -241,23 +240,16 @@ int derp_project_equirect_masks(int device, const DerpCameraDesc* cams, int num_
   }
   if (int rc = upload(s.masks, m.data(), num_cams)) return rc;
   if (int rc = upload(s.maskOuts, outs.data(), num_cams)) return rc;
-  CU(s.hits.ensure(1));
-  CU(s.undecided.ensure(kUndecidedCapacity));
   const dim3 block(derp::sweep::kSweepThreadsX, derp::sweep::kSweepThreadsY);
   const dim3 grid((maxW + block.x - 1) / block.x, (maxH + block.y - 1) / block.y, num_cams);
-  unsigned long long count = 0;
-  for (;;) {  // a second launch only when the undecided list overflowed (the kernel's decisions are deterministic)
-    CU(cudaMemset(s.hits.p, 0, sizeof(unsigned long long)));
-    derp::sweep::projectMasksKernel<<<grid, block>>>(s.cams.p, s.masks.p, depth, s.maskOuts.p, s.undecided.p,
-                                                     s.undecided.n, s.hits.p);
-    CU(cudaGetLastError());
-    CU(cudaMemcpy(&count, s.hits.p, sizeof count, cudaMemcpyDeviceToHost));
-    if (count <= s.undecided.n) break;
-    CU(s.undecided.ensure(count));
-  }
+  std::vector<unsigned long long> list;
+  auto launch = [&](UndecidedView<unsigned long long> undecided) {
+    derp::sweep::projectMasksKernel<<<grid, block>>>(s.cams.p, s.masks.p, depth, s.maskOuts.p, undecided);
+    return DERP_OK;
+  };
+  if (int rc = s.undecided.collect(launch, list)) return rc;
+  const size_t count = list.size();
   if (count) {
-    std::vector<unsigned long long> list(count);
-    CU(cudaMemcpy(list.data(), s.undecided.p, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     std::vector<long long> at(count);
     for (size_t k = 0; k < count; ++k) {
       const int i = (int)(list[k] >> 32);
@@ -265,8 +257,8 @@ int derp_project_equirect_masks(int device, const DerpCameraDesc* cams, int num_
       at[k] = projectPixelHost(c[i], (int)(pixel % W[i]), (int)(pixel / W[i]), depth, m[i].w, m[i].h);
     }
     if (int rc = upload(s.resolved, at.data(), count)) return rc;
-    derp::sweep::resolveMasksKernel<<<(unsigned)((count + 255) / 256), 256>>>(s.masks.p, s.maskOuts.p, s.undecided.p,
-                                                                              s.resolved.p, (int)count);
+    derp::sweep::resolveMasksKernel<<<grid1(count), 256>>>(s.masks.p, s.maskOuts.p, s.undecided.items.p, s.resolved.p,
+                                                           (int)count);
     CU(cudaGetLastError());
   }
   for (int i = 0; i < num_cams; ++i)

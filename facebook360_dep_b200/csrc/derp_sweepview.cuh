@@ -20,6 +20,7 @@
 #include <cstdint>
 
 #include "derp_camera.cuh"
+#include "derp_host.cuh"
 #include "derp_interval.cuh"
 
 namespace derp {
@@ -282,7 +283,7 @@ __device__ __forceinline__ long long eqrIndexProven(const Iv* w, int W, int H) {
 // the reference skips the pixel; undecided pixels are written 1 and listed (camera << 32 | pixel) for the host
 __global__ void __launch_bounds__(kSweepThreadsX * kSweepThreadsY) projectMasksKernel(
     const DevCamera* __restrict__ gCams, const EqrMask* __restrict__ masks, double depth, uint8_t* const* outs,
-    unsigned long long* __restrict__ undecided, unsigned long long capacity, unsigned long long* __restrict__ count) {
+    UndecidedView<unsigned long long> undecided) {
   __shared__ DevCamera cam;
   const int i = blockIdx.z;
   if (threadIdx.x == 0 && threadIdx.y == 0) cam = gCams[i];
@@ -299,8 +300,7 @@ __global__ void __launch_bounds__(kSweepThreadsX * kSweepThreadsY) projectMasksK
     v = m.p[at] ? 255 : 0;
   } else if (at == -2) {
     v = 1;
-    const unsigned long long slot = atomicAdd(count, 1ull);
-    if (slot < capacity) undecided[slot] = (unsigned long long)i << 32 | (unsigned)(y * W + x);
+    undecided.append((unsigned long long)i << 32 | (unsigned)(y * W + x));
   }
   outs[i][(size_t)y * W + x] = v;
 }
