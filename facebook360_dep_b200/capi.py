@@ -353,6 +353,39 @@ class Blur(_Binding):
         return out
 
 
+# ---- include/derp_resize.h ----------------------------------------------------------------------------------------
+_RESIZE_SIGS = {
+    "derp_last_error": (C.c_char_p, []),
+    "derp_resize_area": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                   C.c_int]),
+}
+RESIZE_SYMBOLS = ["derp_resize_area"]
+RESIZE_DTYPES = {np.dtype(np.uint8): 8, np.dtype(np.uint16): 16, np.dtype(np.float32): 32}
+
+
+class Resize(_Binding):
+    """ctypes binding of include/derp_resize.h on a loaded library: ``Resize(load_cuda())``."""
+
+    def __init__(self, library):
+        self.path, self.lib = _bind(library, _RESIZE_SIGS)
+
+    check = _Binding._check
+
+    def resize_area(self, image, out_w, out_h, threshold=None, device=0):
+        """cv2.resize(image, (out_w, out_h), interpolation=INTER_AREA) [then cv2.threshold(., threshold, 255,
+        THRESH_BINARY)] of a uint8, uint16 or float32 HxW or HxWxC image, C = 1, 3 or 4; the result has image's layout."""
+        image = np.ascontiguousarray(image)
+        bits = RESIZE_DTYPES.get(image.dtype)
+        if bits is None:
+            raise ValueError("resize_area: uint8, uint16 or float32 samples, not %s" % image.dtype)
+        h, w = image.shape[:2]
+        c = image.shape[2] if image.ndim == 3 else 1
+        out = np.empty((out_h, out_w) + image.shape[2:], image.dtype)
+        self.check(self.lib.derp_resize_area(device, image.ctypes.data, bits, c, w, h, out.ctypes.data, out_w, out_h,
+                                             -1 if threshold is None else int(threshold)))
+        return out
+
+
 # ---- include/derp_rephoto.h ---------------------------------------------------------------------------------------
 _REPHOTO_SIGS = {
     "derp_last_error": (C.c_char_p, []),

@@ -4,6 +4,7 @@
 // stand-alone depth stages; derp_convert.cu, derp_canopy.cu and derp_sweepview.cu hold the other entry points.
 //
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see Makefile).
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -12,9 +13,11 @@
 #include <memory>
 
 #include "../../include/derp_blur.h"
+#include "../../include/derp_resize.h"
 #include "derp_host.cuh"
 #include "derp_kernels.cuh"
 #include "derp_refine.cuh"
+#include "derp_resize.cuh"
 
 using namespace derp;
 
@@ -1159,9 +1162,8 @@ int derp_upsample_from_kept(DerpCtx* c, int dst, const uint8_t* coarse_mask, con
                            "derp_upsample_from_kept");
 }
 
-// computeResizeAreaTab (resize.cpp) as per-destination tap ranges
-static void areaTaps(int ssize, int dsize, std::vector<int>& ofs, std::vector<int>& si, std::vector<float>& alpha) {
-  const double scale = (double)ssize / dsize;
+// computeResizeAreaTab (resize.cpp) as per-destination tap ranges; scale = 1. / (dsize / ssize), as cv::resize derives it
+static void areaTaps(int ssize, int dsize, double scale, std::vector<int>& ofs, std::vector<int>& si, std::vector<float>& alpha) {
   ofs.assign(1, 0);
   si.clear();
   alpha.clear();
@@ -1187,6 +1189,105 @@ static void areaTaps(int ssize, int dsize, std::vector<int>& ofs, std::vector<in
   }
 }
 
+// The taps of INTER_AREA's bilinear variant on one axis (cv::resize when an axis grows).  On the x axis a column whose
+// second tap would pass the last one takes the last column alone (xmax: the first such column); rows are clipped by the
+// kernel instead, with the weights as computed.
+static void linearTaps(int ssize, int dsize, bool xAxis, std::vector<LinearTap>& tab, int* xmax) {
+  const double inv = (double)dsize / ssize, scale = 1. / inv;
+  tab.resize(dsize);
+  if (xmax) *xmax = dsize;
+  for (int d = 0; d < dsize; ++d) {
+    int s = floorD(d * scale);
+    float f = (float)((d + 1) - (s + 1) * inv);
+    f = f <= 0 ? 0.f : f - (float)floorD(f);
+    if (xAxis && s + 1 >= ssize) {
+      *xmax = std::min(*xmax, d);
+      if (s >= ssize - 1) {
+        f = 0.f;
+        s = ssize - 1;
+      }
+    }
+    const float w0 = 1.f - f;
+    tab[d] = LinearTap{s, w0, f, (int)std::lrintf(w0 * (float)kResizeCoefScale), (int)std::lrintf(f * (float)kResizeCoefScale)};
+  }
+}
+
+}  // extern "C"
+
+namespace {
+// grow-only tap tables per host thread
+struct ResizeTables {
+  DevBuf<int> xo, xs, yo, ys;
+  DevBuf<float> xa, ya;
+  DevBuf<LinearTap> xl, yl;
+};
+
+// cv::resize(INTER_AREA) [+ threshold] of device image sp into device image dp on the legacy default stream.  *synced: the
+// call waited for the kernel (a general ratio: its tables live in thread scratch).
+template <typename T, int C>
+int resizeAreaDevice(const T* sp, int sw, int sh, T* dp, int dw, int dh, int thr, ResizeTables& sc, bool* synced) {
+  *synced = false;
+  const size_t nd = (size_t)dw * dh * C;
+  const dim3 grid((unsigned)(((size_t)dw * C + 255) / 256), (unsigned)std::min(dh, 65535));
+  if (sw == dw && sh == dh && thr < 0) {  // cv::resize copies an image of the same size
+    CU(cudaMemcpyAsync(dp, sp, nd * sizeof(T), cudaMemcpyDeviceToDevice, 0));
+    return DERP_OK;
+  }
+  const double scaleX = 1. / ((double)dw / sw), scaleY = 1. / ((double)dh / sh);
+  int rc;
+  if (scaleX >= 1 && scaleY >= 1) {
+    const int kx = (int)std::lrint(scaleX), ky = (int)std::lrint(scaleY);  // saturate_cast<int>
+    if (std::fabs(scaleX - kx) < 2.220446049250313e-16 && std::fabs(scaleY - ky) < 2.220446049250313e-16) {
+      areaResizeFastKernel<T, C><<<grid, 256>>>(sp, sw, dp, dw, dh, kx, ky, thr);
+    } else {
+      std::vector<int> xo, xs, yo, ys;
+      std::vector<float> xa, ya;
+      areaTaps(sw, dw, scaleX, xo, xs, xa);
+      areaTaps(sh, dh, scaleY, yo, ys, ya);
+      if ((rc = upload(sc.xo, xo.data(), xo.size())) || (rc = upload(sc.xs, xs.data(), xs.size())) ||
+          (rc = upload(sc.xa, xa.data(), xa.size())) || (rc = upload(sc.yo, yo.data(), yo.size())) ||
+          (rc = upload(sc.ys, ys.data(), ys.size())) || (rc = upload(sc.ya, ya.data(), ya.size())))
+        return rc;
+      areaResizeKernel<T, C><<<grid, 256>>>(sp, sw, dp, dw, dh, sc.xo.p, sc.xs.p, sc.xa.p, sc.yo.p, sc.ys.p, sc.ya.p, thr);
+      CU(cudaDeviceSynchronize());
+      *synced = true;
+    }
+  } else {
+    std::vector<LinearTap> xt, yt;
+    int xmax = 0;
+    linearTaps(sw, dw, true, xt, &xmax);
+    linearTaps(sh, dh, false, yt, nullptr);
+    if ((rc = upload(sc.xl, xt.data(), xt.size())) || (rc = upload(sc.yl, yt.data(), yt.size()))) return rc;
+    areaEnlargeKernel<T, C><<<grid, 256>>>(sp, sw, sh, dp, dw, dh, sc.xl.p, xmax, sc.yl.p, thr);
+    CU(cudaDeviceSynchronize());
+    *synced = true;
+  }
+  CU(cudaGetLastError());
+  return DERP_OK;
+}
+
+// derp_resize_area for one sample type and channel count: stage, resize, copy back, return with dst written
+template <typename T, int C>
+int resizeAreaCall(const void* src, int sw, int sh, void* dst, int dw, int dh, int thr) {
+  static thread_local struct {
+    DevBuf<T> src, dst;
+    ResizeTables tables;
+  } sc;
+  const T* sp = static_cast<const T*>(src);
+  T* dp = static_cast<T*>(dst);
+  const size_t ns = (size_t)sw * sh * C, nd = (size_t)dw * dh * C;
+  bool synced = false;
+  int rc = stageIn(sp, ns, sc.src);
+  if (rc || (rc = outBuffer(dp, nd, sc.dst)) || (rc = resizeAreaDevice<T, C>(sp, sw, sh, dp, dw, dh, thr, sc.tables, &synced)) ||
+      (rc = stageOut(static_cast<T*>(dst), dp, nd)))
+    return rc;
+  CU(cudaDeviceSynchronize());
+  return DERP_OK;
+}
+}  // namespace
+
+extern "C" {
+
 int derp_downscale_area(int device, const uint16_t* src, int src_w, int src_h, uint16_t* dst, int dst_w, int dst_h) {
   if (!src || !dst || src_w < 1 || src_h < 1 || dst_w < 1 || dst_h < 1 || dst_w > src_w || dst_h > src_h)
     return fail(DERP_EINVAL, "derp_downscale_area: bad arguments (INTER_AREA is only used to shrink on this path)");
@@ -1195,38 +1296,46 @@ int derp_downscale_area(int device, const uint16_t* src, int src_w, int src_h, u
   // grow-only scratch per host thread: staged images and the tap tables of a general ratio
   static thread_local struct {
     DevBuf<uint16_t> src, dst;
-    DevBuf<int> xo, xs, yo, ys;
-    DevBuf<float> xa, ya;
+    ResizeTables tables;
   } sc;
   // device-resident images are used in place; host images are staged
   const uint16_t* sp = src;
   uint16_t* dp = dst;
   int rc = stageIn(sp, ns, sc.src);
   if (rc || (rc = outBuffer(dp, nd, sc.dst))) return rc;
-  const double sx = (double)src_w / dst_w, sy = (double)src_h / dst_h;
-  const int kx = (int)std::floor(sx + 0.5), ky = (int)std::floor(sy + 0.5);
-  const dim3 grid((dst_w * 3 + 255) / 256, dst_h);
-  if (std::fabs(sx - kx) < 2.220446049250313e-16 && std::fabs(sy - ky) < 2.220446049250313e-16) {
-    // stream-ordered on the legacy default stream when both images are device memory (a pyramid built on the device)
-    areaResizeFastKernel<<<grid, 256>>>(sp, src_w, dp, dst_w, dst_h, kx, ky);
-  } else {
-    std::vector<int> xo, xs, yo, ys;
-    std::vector<float> xa, ya;
-    areaTaps(src_w, dst_w, xo, xs, xa);
-    areaTaps(src_h, dst_h, yo, ys, ya);
-    if ((rc = upload(sc.xo, xo.data(), xo.size())) || (rc = upload(sc.xs, xs.data(), xs.size())) ||
-        (rc = upload(sc.xa, xa.data(), xa.size())) || (rc = upload(sc.yo, yo.data(), yo.size())) ||
-        (rc = upload(sc.ys, ys.data(), ys.size())) || (rc = upload(sc.ya, ya.data(), ya.size())))
-      return rc;
-    areaResizeKernel<<<grid, 256>>>(sp, src_w, src_h, dp, dst_w, dst_h, sc.xo.p, sc.xs.p, sc.xa.p, sc.yo.p, sc.ys.p,
-                                    sc.ya.p);
-    CU(cudaDeviceSynchronize());  // a general ratio returns with dst written
-  }
-  CU(cudaGetLastError());
+  // an integer ratio is stream-ordered on the legacy default stream when both images are device memory (a pyramid built
+  // on the device); a general ratio returns with dst written
+  bool synced = false;
+  if ((rc = resizeAreaDevice<uint16_t, 3>(sp, src_w, src_h, dp, dst_w, dst_h, -1, sc.tables, &synced))) return rc;
   if ((rc = stageOut(dst, dp, nd))) return rc;
   // a staged image returns with the copies done: the caller may reuse its buffer (a copy to another GPU does not wait)
   if (sp != src || dp != dst) CU(cudaDeviceSynchronize());
   return DERP_OK;
+}
+
+int derp_resize_area(int device, const void* src, int sample_bits, int channels, int src_w, int src_h, void* dst, int dst_w,
+                     int dst_h, int threshold) {
+  if (!src || !dst || (sample_bits != 8 && sample_bits != 16 && sample_bits != 32) ||
+      (channels != 1 && channels != 3 && channels != 4) || src_w < 1 || src_h < 1 || dst_w < 1 || dst_h < 1)
+    return fail(DERP_EINVAL, "derp_resize_area: bad arguments (8-, 16- or 32-bit samples, 1, 3 or 4 channels, sizes > 0)");
+  // rows of samples are indexed with int and whole images with size_t
+  size_t bytes;
+  for (const auto& [w, h] : {std::pair<int, int>{src_w, src_h}, {dst_w, dst_h}})
+    if ((size_t)w * channels > (size_t)INT_MAX ||
+        __builtin_mul_overflow((size_t)w * channels * (sample_bits / 8), (size_t)h, &bytes))
+      return fail(DERP_EINVAL, "derp_resize_area: image too large");
+  CU(cudaSetDevice(device));
+  switch (sample_bits * 8 + channels) {
+    case 8 * 8 + 1: return resizeAreaCall<uint8_t, 1>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 8 * 8 + 3: return resizeAreaCall<uint8_t, 3>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 8 * 8 + 4: return resizeAreaCall<uint8_t, 4>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 16 * 8 + 1: return resizeAreaCall<uint16_t, 1>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 16 * 8 + 3: return resizeAreaCall<uint16_t, 3>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 16 * 8 + 4: return resizeAreaCall<uint16_t, 4>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 32 * 8 + 1: return resizeAreaCall<float, 1>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    case 32 * 8 + 3: return resizeAreaCall<float, 3>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+    default: return resizeAreaCall<float, 4>(src, src_w, src_h, dst, dst_w, dst_h, threshold);
+  }
 }
 
 int derp_device_alloc(int device, size_t bytes, void** out) {
